@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Headline benchmark: heads/sec at 256x256 (image -> 413 FLAME params -> 5023x3 vertices -> projected landmarks).
 
-    python bench.py --gpus N --steps K --warmup W                    # this repo (B200-native path), BASELINE configs[1]
+    python bench.py --gpus N --steps K --warmup W                    # this repo (H100-native path), BASELINE configs[1]
     python bench.py --impl reference --gpus N --steps K --warmup W   # the UNMODIFIED reference code on the host CPU cores
     python bench.py --config {2,3,4,5}                               # other BASELINE.json configs (1-based, as SURVEY §8d)
 
@@ -98,13 +98,14 @@ def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         d = json.load(open(p))
-        return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "bf16_tflops": d.get("bf16_tflops", 1590.0),
-                "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+        return {"hbm_gbs": d.get("hbm_gbs", 3350.0), "bf16_tflops": d.get("bf16_tflops", 989.0),
+                "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 989.0), "source": "measured"}
+    # NVIDIA H100 SXM data sheet (dense, 700 W card); a power-limited card reaches less
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -313,6 +314,11 @@ def run_ours(args):
     torch.cuda.synchronize()
     launches_per_step = _lib.launch_count() - launches0      # a graph replay launches the same kernels (counted at capture)
     ms_total = timed(dev_stream, x_dev, args.steps)          # EXACTLY K steps -> `value`
+    # what the last timed step returned (its slot's device outputs stay valid until that slot is submitted again)
+    last_out = None
+    if args.dump_outputs:
+        last = dev_stream.slots[(dev_stream._head - 1) % dev_stream.depth]["out"]
+        last_out = {k: last[k].detach().to("cpu", torch.float32) for k in keys}
     # a region of >= 1.5 s of the same steps: settled clocks, enough nvidia-smi samples; reported beside the K-step number
     per_step = ms_total / args.steps
     n_long = max(args.steps, int(1500.0 / max(per_step, 1e-3)) + 1) if not args.quick else args.steps
@@ -392,7 +398,7 @@ def run_ours(args):
                     "parallelism": (f"dp{world} (batch sharded, NCCL bcast constants at start-up, per-step all-gather of params/"
                                     f"vertices/landmarks on a side stream overlapping the next step)") if distributed
                     else "single GPU",
-                    "l2": "no explicit flush: per-step working set (50 MB input + >1 GB activations) exceeds the 126 MB L2"})
+                    "l2": "no explicit flush: per-step working set (50 MB input + >1 GB activations) exceeds the 50 MB L2"})
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": n_warm, "ms_per_step": ms_total / args.steps, "higher_is_better": True,
@@ -412,7 +418,7 @@ def run_ours(args):
             "launch_mode": "CUDA graph replay of FaceMeshPredictor.predict_batch (one graph launch per step; gpu_launches = "
                            "kernels inside the graph x steps)",
             "clocks": clocks,
-            "roofline": {"kernel": "tile_gemm_kernel<EpiConv> (all conv/linear layers, tcgen05)", "bound": "tensor",
+            "roofline": {"kernel": "tile_gemm_kernel<EpiConv> (all conv/linear layers, wgmma)", "bound": "tensor",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if peak else None,
                          "traffic": traffic if B == 64 and args.precision == "fp16x2" else None,
                          "traffic_unit": "DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum, averaged "
@@ -466,9 +472,33 @@ def run_ours(args):
             line["parity"] = cb.pop("parity", None)
             line["cpu_baseline"] = cb
         print(json.dumps(line), flush=True)
+    if last_out is not None and rank == 0:
+        dump_outputs(args.dump_outputs, last_out)
     if distributed:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, outputs):
+    """Write each output as out_dir/<name>.npy (float32).  Above DUMP_LIMIT_BYTES in all, the same fixed, seeded sample of
+    batch rows is kept from every output, so two builds can still be compared row for row."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() * 4 for t in outputs.values())
+    B = next(iter(outputs.values())).shape[0]
+    rows = None
+    if total > DUMP_LIMIT_BYTES:
+        keep = max(1, B * DUMP_LIMIT_BYTES // total)
+        rows = torch.randperm(B, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        np.save(os.path.join(out_dir, "sample_rows.npy"), rows.numpy().astype(np.float64))
+    for k, t in outputs.items():
+        if rows is not None:
+            t = t[rows]
+        np.save(os.path.join(out_dir, f"{k}.npy"), t.numpy().astype(np.float32))
 
 
 def sub_pipeline(FaceMeshPredictor, DEFAULT_CONFIG, sd, static, local_rank, B, precision, timed, group, world, what):
@@ -616,12 +646,17 @@ def main():
     ap.add_argument("--quick", action="store_true", help="profiling aid (ncu launch lists): no >= 1.5 s region, no sub-objects, "
                     "no strict-mode run, no CPU baseline -- only warm-up + the K timed steps of both arms")
     ap.add_argument("--workload", default=None, choices=["pipeline", "decode"], help="legacy alias: decode = --config 5")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32, <= 64 MB; "
+                         "inputs are seeded, so two builds can be compared output for output)")
     args = ap.parse_args()
     if args.workload == "decode":
         args.config = 5
     args = resolve(args)
     if args.quick:
         args.no_extras = args.no_strict = args.no_cpu_baseline = True
+    if args.dump_outputs and (args.impl == "reference" or args.config == 5):
+        ap.error("--dump-outputs applies to the pipeline workload of this implementation (configs 2-4)")
     if args.impl == "reference":
         run_reference(args)
     elif args.config == 5:

@@ -1,8 +1,8 @@
-"""dad_3dheads_b200 -- B200-native (sm_100a) DAD-3DNet image->3D-head hot path.
+"""dad_3dheads_b200 -- H100-native (sm_90a) DAD-3DNet image->3D-head hot path.
 
 Host side is Python/PyTorch (device memory, streams, torch.distributed); all arithmetic on the path runs in
 hand-written CUDA behind the C ABI of ``libdad3d.so`` (include/dad3d.h).  There is no CPU fallback: importing the
-compute classes without the built library, or calling them without a Blackwell GPU, raises.
+compute classes without the built library, or calling them without a Hopper GPU, raises.
 """
 from .flame import FLAME_CONSTS, FlameParams, FLAMELayer  # noqa: F401
 from .head_mesh import HeadMesh  # noqa: F401

@@ -1,7 +1,7 @@
-// DAD-3DNet encoder (FlameRegression.forward, model_training/model/flame_regression.py:87-106) for sm_100a.
+// DAD-3DNet encoder (FlameRegression.forward, model_training/model/flame_regression.py:87-106) for sm_90a.
 // Host side: folded weights -> bf16 piece planes + TMA maps (create), a per-batch-size execution plan with a
 // liveness-based workspace layout (plan), and the launch loop (forward).  Device side: tile_gemm.cuh (every conv /
-// linear layer as an implicit GEMM on tcgen05) + encoder_kernels.cuh (stem, pooling, BiFPN sums, fusion concat, heads).
+// linear layer as an implicit GEMM on wgmma) + encoder_kernels.cuh (stem, pooling, BiFPN sums, fusion concat, heads).
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -44,7 +44,7 @@ struct ConvW {
 int pick_block_n(int cout) {
   if (cout % 128 == 0) return 128;
   if (cout % 64 == 0) return 64;
-  if (cout <= 80) return 80;                  // heat-map head: 68 -> one 80-wide tile (UMMA N % 16 == 0)
+  if (cout <= 80) return 80;                  // heat-map head: 68 -> one 80-wide tile (wgmma N % 8 == 0)
   return 96;                                  // 549 -> 6 x 96
 }
 
@@ -131,9 +131,7 @@ struct dad3d_encoder {
   bool kernels_configured = false, stem_configured = false;   // cudaFuncSetAttribute done on this handle's device
   bool td_parity = false;          // env DAD3D_TD_PARITY=1: large top-down nodes as four parity launches
   bool heat_sparse = true;         // env DAD3D_HEAT_SPARSE=0: always compute the full heat-map
-  bool use_pair = false;           // env DAD3D_PAIR=1: cta_group::2 CTA pairs for the large 128-wide layers
-  bool use_pdl = false;            // programmatic dependent launch for the tile-engine kernels (env DAD3D_PDL=1 enables;
-                                   // measured neutral on B200 at batch 64: 6689 vs 6764 heads/s, so off by default)
+  bool use_pdl = false;            // programmatic dependent launch for the tile-engine kernels (env DAD3D_PDL=1 enables)
   bool debug_keep_all = false;     // disable buffer reuse so every activation can be read back after a forward
   // live profiling of the dominant kernel (bench.py roofline): CUDA events around every tile_gemm launch
   bool profile = false;
@@ -512,7 +510,10 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     const bool res_in_k = s.res >= 0 && s.res_mode == 1 && w->has_identity;
     // few row tiles (small maps / small batch): halve the tile width so that twice as many CTAs share the work
     const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
-    const bool narrow = w->has_b64 && m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms;
+    GemmGeom fit;                                     // the full-width tile needs a two-deep operand ring in shared memory
+    std::memset(&fit, 0, sizeof(fit));
+    fit.nA = enc->P; fit.nB = enc->P; fit.block_n = w->block_n;
+    const bool narrow = w->has_b64 && (m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms || gemm_max_stages(fit) < 2);
     const int block_n = narrow ? 64 : w->block_n;
     g.block_n = block_n;
     g.n_tiles = w->cout_pad / block_n;
@@ -534,10 +535,6 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
       g.res_kind = 1;
       g.res_stride = s.res_stride;
     }
-    // CTA pairs (cta_group::2): each CTA of a pair loads only half of the B tile; worth it when every SM pair has work
-    const bool pair = enc->use_pair && block_n == 128 && w->has_b64 &&
-                      ((m_tiles + 1) / 2) * g.n_tiles >= enc->num_sms / 2;
-    g.pair = (pair && !halo) ? 1 : 0;
     g.stages = gemm_max_stages(g);
     if (halo) {
       g.halo = 1;
@@ -549,7 +546,8 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
       g.stages_b = gemm_halo_b_stages(g);
       if (g.stages_b < 2) { set_error("layer " + w->name + ": halo pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
     }
-    if (g.stages < 2) { set_error("layer " + w->name + ": pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
+    // (the 80 / 96-wide heads at three pieces fit one operand stage only: the producer then refills behind each k-block)
+    if (g.stages < 1) { set_error("layer " + w->name + ": pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
     for (int p = 0; p < enc->P; ++p) {
       // stem: row x of the A operand is the 64-element window that starts at padded s2d pixel x (dim 1 advances by one
       // 16-channel pixel = 32 bytes while the window is 128 bytes long: consecutive rows overlap)
@@ -562,7 +560,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
       const uint32_t es[4] = {1, static_cast<uint32_t>(s.stride), static_cast<uint32_t>(s.stride), 1};
       const uint16_t* basep = reinterpret_cast<const uint16_t*>(ti.ptr) + static_cast<size_t>(p) * ti.plane_elems();
       if (!make_tmap_16bit(&s.maps.a[p], basep, 4, dims, strides, box, es)) return DAD3D_ERR_CUDA;
-      s.maps.b[p] = (narrow || g.pair || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];    // pair: each CTA loads a 64-row half of the B tile
+      s.maps.b[p] = (narrow || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];
     }
     if (res_in_k || src2) {
       const TensorInfo& tr = plan->tensors[s.res];
@@ -659,16 +657,14 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
   if (!enc->kernels_configured) {                  // function attributes are per device: remembered per handle
     DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConv>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
     DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConvH>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConvH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConv, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
     enc->kernels_configured = true;
   }
   const GemmGeom& g = s.geom;
   const int m_tiles_total = g.tiles_w * g.tiles_h * g.tiles_n;
-  const int total = g.pair ? ((m_tiles_total + 1) / 2) * g.n_tiles * 2 : m_tiles_total * g.n_tiles;
-  int grid = g.pair ? std::min(total, enc->num_sms & ~1) : std::min(total, enc->num_sms);
-  const int csz = g.pair ? 2 : g.cl_m * g.cl_n;
-  if (!g.pair && csz > 1) grid = std::min(((m_tiles_total + g.cl_m - 1) / g.cl_m) * csz, (enc->num_sms / csz) * csz);
+  const int total = m_tiles_total * g.n_tiles;
+  int grid = std::min(total, enc->num_sms);
+  const int csz = g.cl_m * g.cl_n;
+  if (csz > 1) grid = std::min(((m_tiles_total + g.cl_m - 1) / g.cl_m) * csz, (enc->num_sms / csz) * csz);
   std::pair<cudaEvent_t, cudaEvent_t>* ev = nullptr;
   if (enc->profile) {
     if (enc->prof_used == enc->prof_events.size()) {
@@ -705,13 +701,8 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    if (g.pair) {
-      if (enc->fp16) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConvH, true>, s.maps, g, s.epi));
-      else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConv, true>, s.maps, g, s.epi));
-    } else {
-      if (enc->fp16) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConvH>, s.maps, g, s.epi));
-      else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConv>, s.maps, g, s.epi));
-    }
+    if (enc->fp16) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConvH>, s.maps, g, s.epi));
+    else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConv>, s.maps, g, s.epi));
   }
   count_launch();
   if (ev) DAD3D_CUDA_OK(cudaEventRecord(ev->second, stream));
@@ -733,8 +724,8 @@ int dad3d_encoder_create(dad3d_encoder** out, const dad3d_conv_weights* layers, 
   DAD3D_CUDA_OK(cudaSetDevice(device));
   cudaDeviceProp prop;
   DAD3D_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("libdad3d requires an sm_100 (Blackwell) device");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libdad3d requires an sm_90 (Hopper) device");
     return DAD3D_ERR_UNSUPPORTED;
   }
   std::unique_ptr<dad3d_encoder> enc(new dad3d_encoder());
@@ -766,8 +757,6 @@ int dad3d_encoder_create(dad3d_encoder** out, const dad3d_conv_weights* layers, 
     enc->td_parity = (e6 && e6[0] == '1');
     const char* e9 = std::getenv("DAD3D_HEAT_SPARSE");
     enc->heat_sparse = !(e9 && std::atoi(e9) == 0);
-    const char* e3 = std::getenv("DAD3D_PAIR");
-    enc->use_pair = (e3 && e3[0] == '1');
     const char* e2 = std::getenv("DAD3D_STEM_SIMT");
     enc->stem_simt = (e2 && e2[0] == '1');
   }

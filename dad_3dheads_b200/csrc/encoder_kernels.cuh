@@ -1,4 +1,4 @@
-// Device code of the DAD-3DNet encoder (everything that is not the tcgen05 tile engine itself):
+// Device code of the DAD-3DNet encoder (everything that is not the wgmma tile engine itself):
 //   EpiConv            fused conv epilogue: folded-BN bias, residual add / gate multiply, ReLU, split into bf16 pieces
 //   stem_conv_kernel   7x7/2 conv (Cin = 3) + folded BN + ReLU, fp32 CUDA cores, NCHW fp32 image -> NHWC fp32 (DAD3D_STEM_SIMT=1)
 //   stem_s2d_kernel    2x2 space-to-depth + piece split of the image: the stem runs on the tile engine as a 4x4 conv
@@ -131,7 +131,8 @@ struct EpiConvParams {
 template <bool F16>
 struct EpiConvT {
   static constexpr int kExtraSmemBytes = 0;
-  struct State {
+  struct State {};
+  struct Res {
     float r[64];              // residual / gate operand of the current tile (this thread's row, this warp's columns)
   };
   using Params = EpiConvParams;
@@ -139,13 +140,11 @@ struct EpiConvT {
   static __device__ __forceinline__ void run_f32(const Params& ep, const EpiCtx& c) {
     int cb, ce;
     epi_chunk_range(*c.g, c.grp, &cb, &ce);
-    if (cb >= ce) epi_release_tmem(c);
     for (int ch = cb; ch < ce; ++ch) {
       float x[32];
       const bool tail16 = ch * 32 + 32 > c.g->block_n;            // 16-column last chunk (block_n = 80)
       if (tail16) epi_load16<0>(c, ch * 32, x);
       else epi_load32<0>(c, ch * 32, x);
-      if (ch == ce - 1) epi_release_tmem(c);
       if (!c.valid) continue;
       const int col = c.col0 + ch * 32;
       float4* d = reinterpret_cast<float4*>(ep.out_f32 + c.pix * ep.ld_f32 + col);
@@ -177,12 +176,11 @@ struct EpiConvT {
     return c.grp * (c.g->block_n / 2) + half * 32;            // column inside the tile
   }
 
-  // Residual / gate operand: the warp's 32 rows x 32 channels per piece plane, loaded BEFORE the accumulator is awaited
-  // so the latency hides behind the tile's main loop.  Loads are cooperative (a warp instruction covers whole 64-byte
+  // Residual / gate operand: the warp's 32 rows x 32 channels per piece plane.  Loads are cooperative (a warp instruction covers whole 64-byte
   // row segments -> 8 memory wavefronts instead of 32 for per-thread rows), transposed through the staging tile; every
   // lane then reads back its own row and sums the pieces (smallest first).
   template <int H>
-  static __device__ __forceinline__ void prefetch_half(const Params& ep, const EpiCtx& c, State& st) {
+  static __device__ __forceinline__ void prefetch_half(const Params& ep, const EpiCtx& c, Res& st) {
     const int swz = (c.lane >> 1) & 3;
     const uint8_t* rowp = c.stage + c.lane * 64;
     const int col = c.col0 + first_col(c, H);
@@ -232,18 +230,14 @@ struct EpiConvT {
     }
   }
 
-  static __device__ __forceinline__ void prefetch(const Params& ep, EpiCtx& c, State& st) {
-    if (ep.res_mode == 0 || ep.out == nullptr) return;
-    prefetch_half<0>(ep, c, st);
-    if (halves(c) == 2) prefetch_half<1>(ep, c, st);
-  }
+  // (the residual is loaded inside run(): a per-tile register array kept out of the main loop, where the accumulators live)
+  static __device__ __forceinline__ void prefetch(const Params&, EpiCtx&, State&) {}
 
   template <int H>
-  static __device__ __forceinline__ void run_half(const Params& ep, const EpiCtx& c, State& st, bool last) {
+  static __device__ __forceinline__ void run_half(const Params& ep, const EpiCtx& c, Res& st) {
     float x[32];
     const int colt = first_col(c, H);
     epi_load32<0>(c, colt, x);
-    if (last) epi_release_tmem(c);
     const int col = c.col0 + colt;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -300,14 +294,19 @@ struct EpiConvT {
     }
   }
 
-  static __device__ __forceinline__ void run(const Params& ep, EpiCtx& c, State& st) {
+  static __device__ __forceinline__ void run(const Params& ep, EpiCtx& c, State&) {
+    Res st;
+    if (ep.res_mode != 0 && ep.out != nullptr) {
+      prefetch_half<0>(ep, c, st);
+      if (halves(c) == 2) prefetch_half<1>(ep, c, st);
+    }
     if (ep.out == nullptr) {
       run_f32(ep, c);
     } else if (halves(c) == 2) {
-      run_half<0>(ep, c, st, false);
-      run_half<1>(ep, c, st, true);
+      run_half<0>(ep, c, st);
+      run_half<1>(ep, c, st);
     } else {
-      run_half<0>(ep, c, st, true);
+      run_half<0>(ep, c, st);
     }
   }
 };
@@ -318,7 +317,7 @@ using EpiConvH = EpiConvT<true>;      // fp16 hi/lo pieces, per-channel weight s
 // 7x7 stride-2 pad-3 conv, 3 -> 64 channels, BN folded, ReLU.  in: NCHW fp32 [B,3,H,W]; out: NHWC fp32 [B,H/2,W/2,64].
 // Block = 16x16 output pixels, 256 threads.  Thread = 4 horizontally adjacent pixels x 16 output channels (warp-uniform
 // channel group, so weight reads are shared-memory broadcasts); per (channel, filter row) the 13 input values the 4 pixels
-// need are loaded once and reused across the 7 filter columns.  fp32 math as packed fma.rn.f32x2 (2 FMAs / instruction).
+// need are loaded once and reused across the 7 filter columns.
 constexpr int kStemTile = 16;
 constexpr int kStemPatch = kStemTile * 2 + 5;    // 37
 constexpr int kStemSmemBytes = (147 * 64 + 3 * kStemPatch * (kStemPatch + 1)) * 4;
@@ -373,7 +372,7 @@ stem_conv_kernel(const float* __restrict__ img, const float* __restrict__ w /*[1
           const float xs = in[2 * p + kx];
           const float2 xv = make_float2(xs, xs);
 #pragma unroll
-          for (int o = 0; o < 8; ++o) acc[p][o] = __ffma2_rn(xv, wv[o], acc[p][o]);
+          for (int o = 0; o < 8; ++o) acc[p][o] = make_float2(fmaf(xv.x, wv[o].x, acc[p][o].x), fmaf(xv.y, wv[o].y, acc[p][o].y));
         }
       }
     }

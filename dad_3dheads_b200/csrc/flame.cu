@@ -1,7 +1,7 @@
-// FLAME head decoder for sm_100a:  413 params -> 5023x3 vertices (+ weak-perspective projection) in three kernels
+// FLAME head decoder for sm_90a:  413 params -> 5023x3 vertices (+ weak-perspective projection) in three kernels
 //   K1 flame_prep_kernel    per-head small math: betas -> fp16 hi/lo coefficient rows, folded joint regression,
 //                           Rodrigues, kinematic chain, 6-DoF rotation folded into the skinning transforms
-//   K2 tile_gemm_kernel<EpiBlend>   blend shapes + pose correctives as ONE tcgen05 GEMM  [heads,448] x [15069,448]^T
+//   K2 tile_gemm_kernel<EpiBlend>   blend shapes + pose correctives as ONE wgmma GEMM  [heads,448] x [15069,448]^T
 //   K3 lbs_project_kernel   linear-blend skinning + z offset + rotation + projection, shared-memory staged, coalesced
 //   K4 gather kernels       landmark subsets
 // Reference math: model_training/model/flame.py:182-229, smplx.lbs (0.1.26), model_training/model/utils.py:92-101,
@@ -223,11 +223,9 @@ struct EpiBlend {
   static __device__ __forceinline__ void run(const Params& ep, EpiCtx& c, State&) {
     int cb, ce;
     epi_chunk_range(*c.g, c.grp, &cb, &ce);
-    if (cb >= ce) epi_release_tmem(c);
     for (int ch = cb; ch < ce; ++ch) {
       float x[32];
       epi_load32<0>(c, ch * 32, x);
-      if (ch == ce - 1) epi_release_tmem(c);
       if (!c.valid) continue;
       float4* dst = reinterpret_cast<float4*>(ep.out + static_cast<size_t>(c.pix) * ep.ld + c.col0 + ch * 32);
 #pragma unroll
@@ -316,24 +314,9 @@ struct EpiLbs {
     const int vb = (c.col0 + colw) / 3;                                          // first vertex of this warp
     const float wl = st.wl;
 
-    // ---- the warp's 48 accumulator columns (16 vertices) -> registers in one go, then hand TMEM back immediately
+    // ---- the warp's 48 accumulator columns (16 vertices) -> registers in one go
     float xa[48];
-    {
-      const uint32_t t = c.t_acc + static_cast<uint32_t>(colw);
-      ptx::tmem_ld_32x32b_x32_f(t, xa);
-      ptx::tmem_ld_32x32b_x16_f(t + 32, xa + 32);
-      if (c.g->n_acc == 2) {
-        float b[48];
-        ptx::tmem_ld_32x32b_x32_f(t + c.g->block_n, b);
-        ptx::tmem_ld_32x32b_x16_f(t + c.g->block_n + 32, b + 32);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 48; ++j) xa[j] += b[j];
-      } else {
-        ptx::tmem_ld_wait();
-      }
-    }
-    epi_release_tmem(c);
+    epi_load<0, 48>(c, colw, xa);
 
 #pragma unroll
     for (int pass = 0; pass < 2; ++pass) {
@@ -514,7 +497,7 @@ __global__ void gather_bary_kernel(const float* __restrict__ src, int B, int nv,
 //     out_v = w_r(v) (A0' p_s + t0) + w_j(v) (A2' p_s + t2) + c        [A'|t], c = F(jaw, rot6, J(beta))  (flame_prep_kernel)
 //     proj  = ((out * sc + (tx, ty, 0)) + 1) * image/2,  sc = max(s + 1, 1e-8)
 // Backward:  g_v = gV + (image/2) sc gP;   dp_s = (w_r A0'^T + w_j A2'^T) g_v;   d coef = Basis_s^T dp_s  -- the dense part,
-// a [heads,15104] x [15104,448] tcgen05 GEMM through the tile engine (fp16 hi/lo operands, 3 products);  the cotangents of
+// a [heads,15104] x [15104,448] wgmma GEMM through the tile engine (fp16 hi/lo operands, 3 products);  the cotangents of
 // (A0', t0, A2', t2, c) are per-head sums over the vertices;  the 24-input function F (Rodrigues, kinematic chain, 6-DoF
 // Gram-Schmidt) is differentiated in forward mode, one input direction per lane, and contracted with those cotangents.
 namespace dad3d {
@@ -796,9 +779,9 @@ using namespace dad3d;
 
 struct dad3d_flame {
   int device = 0;
-  int smem_configured[4] = {0, 0, 0, 0};     // per handle (= per device): max dynamic smem set for <EpiLbs> / <EpiBlend> /
-                                             // flame_decode_kernel<false> / <true>
-  int max_clusters[2] = {0, 0};              // per handle: co-resident clusters (2x2 tile-engine clusters / decode CTA pairs)
+  int smem_configured[3] = {0, 0, 0};        // per handle (= per device): max dynamic smem set for <EpiLbs> / <EpiBlend> /
+                                             // flame_decode_kernel
+  int max_clusters[1] = {0};                 // per handle: co-resident 2x2 tile-engine clusters
   int nv = 0, n3 = 0, npad = 0;
   int num_sms = 0;
   FlameLayoutDev layout{};
@@ -817,7 +800,7 @@ struct dad3d_flame {
   CUtensorMap map_b48[2];                    // box 64 x 48  (fused path, 2x2 clusters: each CTA loads half of a B tile)
   __half* d_basisT[2] = {nullptr, nullptr};  // [kKPad, npad] hi / lo planes (transposed basis) for the backward GEMM (lazy)
   CUtensorMap map_bT[2];                     // box 64 x 64 over the transposed planes
-  CUtensorMap map_dec[2];                    // hi plane, box 64 x 192 (decode kernel) / 64 x 96 (its CTA-pair variant)
+  CUtensorMap map_dec;                       // hi plane, box 64 x 192 (decode kernel)
   int fused_chunk = 0;                       // heads per pass of the fused path: 4 row tiles per SM
 };
 
@@ -866,19 +849,14 @@ int launch_tile_gemm(const GemmMaps& maps, const GemmGeom& g, const typename Epi
   return DAD3D_OK;
 }
 
-template <bool kPair>
-int decode_groups_max(dad3d_flame* h);
-
 // One launch of flame_decode_kernel over `rows` heads whose fp16 coefficient rows (a_hi) and transform records (xf) the prep
 // kernel has written.
-template <bool kPair>
 int launch_flame_decode(dad3d_flame* h, const __half* a_hi, int rows, const float* xf, float* v3, float* pj, int pc,
                         float image_size, cudaStream_t stream) {
-  int* configured = &h->smem_configured[kPair ? 3 : 2];
-  if (!*configured) {
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<kPair, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<kPair, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
-    *configured = 1;
+  if (!h->smem_configured[2]) {
+    DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
+    DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
+    h->smem_configured[2] = 1;
   }
   CUtensorMap map_a;
   {
@@ -891,25 +869,15 @@ int launch_flame_decode(dad3d_flame* h, const __half* a_hi, int rows, const floa
   p.rows = rows;
   p.nv = h->nv;
   p.n_tiles = ceil_div(h->n3, kDecN);
-  const int m_tiles = dec_rows_padded(rows) / kDecBlockM;          // whole permutation blocks: two row tiles per 256 heads
-  p.m_units = kPair ? m_tiles / 2 : m_tiles;
-  const int groups_max = decode_groups_max<kPair>(h);
-  if (groups_max < 1) return DAD3D_ERR_CUDA;
+  p.m_units = dec_rows_padded(rows) / kDecBlockM;                  // whole permutation blocks: two row tiles per 256 heads
+  const int groups_max = h->num_sms;
   // fewer row tiles than SMs: split every row tile's sweep over the vertex tiles so that all SMs get work
   p.splits = p.m_units >= groups_max ? 1 : ceil_div(groups_max, p.m_units);
   if (p.splits > p.n_tiles) p.splits = p.n_tiles;
   const int units = p.m_units * p.splits;
   const int groups = units < groups_max ? units : groups_max;
-  {
-    // ring geometry: k-blocks per slot (fewer, longer slots amortise the per-slot barrier round trip) -- A/B via environment
-    const char* e = std::getenv("DAD3D_DECODE_KBS");
-    int kbs = e ? std::atoi(e) : (kPair ? 2 : 1);
-    if (kbs < 1) kbs = 1;
-    if (kbs > 4) kbs = 4;
-    while (kbs > 1 && dec_max_stages<kPair>(kbs) < 2) --kbs;
-    p.kbs = kbs;
-    p.stages = dec_max_stages<kPair>(kbs);
-  }
+  p.stages = dec_max_stages();
+  if (p.stages < 2) { set_error("decode pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
   p.xf = xf;
   p.w2 = h->d_w2p;
   p.verts3d = v3;
@@ -924,98 +892,15 @@ int launch_flame_decode(dad3d_flame* h, const __half* a_hi, int rows, const floa
   }
   cudaLaunchConfig_t cfg{};
   cfg.blockDim = dim3(kDecThreads);
-  cfg.gridDim = dim3(groups * (kPair ? 2 : 1));
-  cfg.dynamicSmemBytes = dec_smem_bytes<kPair>(p.stages, p.kbs);
+  cfg.gridDim = dim3(groups);
+  cfg.dynamicSmemBytes = dec_smem_bytes(p.stages);
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
   cfg.numAttrs = 0;
-  if (kPair) {
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.numAttrs = 1;
-  }
-  p.prof = nullptr;
-  if (std::getenv("DAD3D_DECODE_PROFILE")) {
-    // diagnostics: the cycle-accounting instantiation, synchronous, table on stderr (never used by the product path)
-    static bool configured[2] = {false, false};
-    if (!configured[kPair ? 1 : 0]) {
-      DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<kPair, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
-      configured[kPair ? 1 : 0] = true;
-    }
-    const int nblk = static_cast<int>(cfg.gridDim.x);
-    const size_t words = static_cast<size_t>(nblk) * 10 * 8;
-    unsigned* d_prof = nullptr;
-    DAD3D_CUDA_OK(cudaMalloc(&d_prof, words * sizeof(unsigned)));
-    DAD3D_CUDA_OK(cudaMemsetAsync(d_prof, 0, words * sizeof(unsigned), stream));
-    p.prof = d_prof;
-    p.proj = nullptr;                                  // the profiled instantiation writes vertices only
-    DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, flame_decode_kernel<kPair, true, false>, map_a, h->map_dec[kPair ? 1 : 0], p));
-    count_launch();
-    DAD3D_CUDA_OK(cudaStreamSynchronize(stream));
-    std::vector<unsigned> hp(words);
-    DAD3D_CUDA_OK(cudaMemcpy(hp.data(), d_prof, words * sizeof(unsigned), cudaMemcpyDeviceToHost));
-    cudaFree(d_prof);
-    double prod[8] = {0}, mma[8] = {0}, epi[8] = {0};
-    int n_mma = 0;
-    for (int b = 0; b < nblk; ++b) {
-      for (int k = 0; k < 8; ++k) prod[k] += hp[(static_cast<size_t>(b) * 10 + 0) * 8 + k];
-      if (hp[(static_cast<size_t>(b) * 10 + 1) * 8 + 7]) {
-        ++n_mma;
-        for (int k = 0; k < 8; ++k) mma[k] += hp[(static_cast<size_t>(b) * 10 + 1) * 8 + k];
-      }
-      for (int w = 2; w < 10; ++w)
-        for (int k = 0; k < 8; ++k) epi[k] += hp[(static_cast<size_t>(b) * 10 + w) * 8 + k] / 8.0;
-    }
-    const double nb = nblk, nm = n_mma > 0 ? n_mma : 1;
-    std::fprintf(stderr,
-                 "[decode profile] rows %d pair %d blocks %d stages %d kbs %d splits %d | cycles per CTA (mean)\n"
-                 "  producer: total %.0f  wait_empty_slot %.0f  wait_tile_release %.0f\n"
-                 "  mma     : total %.0f  tiles %.1f  wait_free_accumulator %.0f  wait_full_slot %.0f  wait_coefficients %.0f (units 0/1/2: %.0f %.0f %.0f)\n"
-                 "  epilogue: total %.0f  tiles %.1f  wait_full_accumulator %.0f  tmem_ld %.0f  math %.0f  stage+store %.0f (mean of 8 warps)\n",
-                 rows, kPair ? 1 : 0, nblk, p.stages, p.kbs, p.splits, prod[7] / nb, prod[0] / nb, prod[1] / nb, mma[7] / nm, mma[6] / nm,
-                 mma[0] / nm, mma[1] / nm, mma[2] / nm, mma[3] / nm, mma[4] / nm, mma[5] / nm, epi[7] / nb, epi[6] / nb, epi[0] / nb, epi[1] / nb, epi[2] / nb, epi[3] / nb);
-    return DAD3D_OK;
-  }
-  if (pj) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, flame_decode_kernel<kPair, false, true>, map_a, h->map_dec[kPair ? 1 : 0], p));
-  else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, flame_decode_kernel<kPair, false, false>, map_a, h->map_dec[kPair ? 1 : 0], p));
+  if (pj) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, flame_decode_kernel<true>, map_a, h->map_dec, p));
+  else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, flame_decode_kernel<false>, map_a, h->map_dec, p));
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
-}
-
-template <>
-int decode_groups_max<false>(dad3d_flame* h) { return h->num_sms; }
-template <>
-int decode_groups_max<true>(dad3d_flame* h) {
-  if (h->max_clusters[1] == 0) {                       // co-resident CTA pairs (GPC packing may leave a few SMs unpaired)
-    if (!h->smem_configured[3]) {
-      if (cudaFuncSetAttribute(flame_decode_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess ||
-          cudaFuncSetAttribute(flame_decode_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit) != cudaSuccess)
-        return 0;
-      h->smem_configured[3] = 1;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.blockDim = dim3(kDecThreads);
-    cfg.gridDim = dim3(h->num_sms / 2 * 2);
-    cfg.dynamicSmemBytes = dec_smem_bytes<true>(dec_max_stages<true>(2), 2);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, flame_decode_kernel<true, false, true>, &cfg) != cudaSuccess || n < 1) {
-      set_error("no co-resident CTA pair fits");
-      return 0;
-    }
-    h->max_clusters[1] = n;
-  }
-  return h->max_clusters[1];
 }
 
 inline unsigned short f32_to_f16_bits(float x) {
@@ -1057,8 +942,8 @@ int dad3d_flame_create(dad3d_flame** out, const float* shapedirs_h, const float*
   DAD3D_CUDA_OK(cudaSetDevice(device));
   cudaDeviceProp prop;
   DAD3D_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("libdad3d requires an sm_100 (Blackwell) device, found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libdad3d requires an sm_90 (Hopper) device, found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
     return DAD3D_ERR_UNSUPPORTED;
   }
 
@@ -1211,9 +1096,7 @@ int dad3d_flame_create(dad3d_flame** out, const float* shapedirs_h, const float*
     const uint64_t dims[2] = {static_cast<uint64_t>(kKPad), static_cast<uint64_t>(ceil_div(n3, kDecN) * kDecN)};
     const uint64_t strides[1] = {static_cast<uint64_t>(kKPad) * 2};
     const uint32_t box192[2] = {kDecBlockK, kDecN};
-    const uint32_t box96h[2] = {kDecBlockK, kDecN / 2};
-    if (!make_tmap_16bit(&h->map_dec[0], h->d_basis_dec, 2, dims, strides, box192, nullptr)) return fail(DAD3D_ERR_CUDA);
-    if (!make_tmap_16bit(&h->map_dec[1], h->d_basis_dec, 2, dims, strides, box96h, nullptr)) return fail(DAD3D_ERR_CUDA);
+    if (!make_tmap_16bit(&h->map_dec, h->d_basis_dec, 2, dims, strides, box192, nullptr)) return fail(DAD3D_ERR_CUDA);
   }
   h->fused_chunk = h->num_sms * kBlockM * 4;
   *out = h;
@@ -1265,14 +1148,6 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
   // default: the dedicated one-product decode kernel (flame_decode.cuh); DAD3D_BLEND_HILO = 3-product hi/lo operands through
   // the tile engine (fp32-class blend product).  DAD3D_BLEND_FAST is the old name of today's default and is accepted as a no-op.
   const bool dedicated = fused && !(flags & DAD3D_BLEND_HILO);
-  bool pair = false;
-  if (dedicated) {
-    // CTA pairs (cta_group::2) for big batches: half the basis bytes through the L2 per SM -- equal on one 75 776-head pass,
-    // 8 % faster sustained over 1 M heads (46.7 vs 43.0 M heads/s).  DAD3D_DECODE_PAIR=0 switches them off (A/B).
-    const char* env = std::getenv("DAD3D_DECODE_PAIR");
-    const int want = (flags & DAD3D_DECODE_PAIR) ? 1 : (env ? std::atoi(env) : 1);
-    pair = want > 0 && ceil_div(B, kDecBlockM) >= 2 * h->num_sms;
-  }
   const int chunk = fused ? h->fused_chunk : kDecodeChunk;
   const int rows_max = B < chunk ? B : chunk;
   uint8_t* ws = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace_d), 1024));
@@ -1298,8 +1173,7 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
       DAD3D_CUDA_OK(cudaGetLastError());
     }
     if (dedicated) {
-      int rc = pair ? launch_flame_decode<true>(h, a_hi, rows, xf, v3, pj, pc, image_size, stream)
-                    : launch_flame_decode<false>(h, a_hi, rows, xf, v3, pj, pc, image_size, stream);
+      int rc = launch_flame_decode(h, a_hi, rows, xf, v3, pj, pc, image_size, stream);
       if (rc != DAD3D_OK) return rc;
     } else if (flags & DAD3D_BLEND_SIMT) {
       dim3 grid(ceil_div(h->npad, 256), rows);
@@ -1308,9 +1182,7 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
       DAD3D_CUDA_OK(cudaGetLastError());
     } else {
       const int block_n = fused ? kFusedBlockN : kBlendBlockN;
-      // big fused passes (>= one row tile per SM): 2x2 thread-block clusters with TMA multicast of both operands
-      // Measured on B200 (profiles/README.md): with 4-CTA clusters L2 sector reads drop only 28 % and the pass gets 17 %
-      // slower (132 of 148 SMs usable, cross-CTA barrier coupling), so clusters are opt-in.
+      // big fused passes (>= one row tile per SM): 2x2 thread-block clusters with TMA multicast of both operands (opt-in)
       const bool clustered = fused && ceil_div(rows, kBlockM) >= h->num_sms && (flags & DAD3D_DECODE_CLUSTER);
       GemmMaps maps;
       std::memset(&maps, 0, sizeof(maps));
@@ -1487,7 +1359,7 @@ int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32
       count_launch();
       DAD3D_CUDA_OK(cudaGetLastError());
     }
-    {   // the dense part: d coef [rows, 448] = D [rows, 15104] x Basis_s [15104, 448]   (tcgen05, fp16 hi/lo, 3 products)
+    {   // the dense part: d coef [rows, 448] = D [rows, 15104] x Basis_s [15104, 448]   (wgmma, fp16 hi/lo, 3 products)
       GemmMaps maps;
       std::memset(&maps, 0, sizeof(maps));
       __half* planes[2] = {d_hi, d_lo};

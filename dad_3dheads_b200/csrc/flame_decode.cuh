@@ -1,45 +1,33 @@
-// Dedicated FLAME decode kernel for sm_100a (the default path of dad3d_flame_decode):
+// Dedicated FLAME decode kernel for sm_90a (the default path of dad3d_flame_decode):
 //
 //   vertices[h, v, :] = skin( T + S beta_h + P theta_h )                 flame.py:182-229, smplx.lbs, model/utils.py:92-101
 //
-// as ONE persistent tcgen05 kernel: blend shapes + pose correctives + template as a [heads,448] x [15069,448]^T fp16 GEMM
-// (fp32 accumulate in TMEM; the template rides in two K columns and is exact to 22 bits), followed in the epilogue by
-// linear-blend skinning, the z offset, the 6-DoF rotation and the weak-perspective projection (head_mesh.py:33-46), written
-// straight into the reference's [B,5023,3] / [B,5023,2|3] layouts.
+// as ONE persistent wgmma kernel: blend shapes + pose correctives + template as a [heads,448] x [15069,448]^T fp16 GEMM
+// (fp32 accumulate; the template rides in two K columns and is exact to 22 bits), followed in the epilogue by linear-blend
+// skinning, the z offset, the 6-DoF rotation and the weak-perspective projection (head_mesh.py:33-46), written straight into
+// the reference's [B,5023,3] / [B,5023,2|3] layouts.
 //
-// Why not the generic tile engine (tile_gemm.cuh, still used by the strict hi/lo mode): measured there, the main loop is
-// bound by SHARED-MEMORY bandwidth, not by the tensor pipe -- every k-block re-streams the 128-head coefficient tile
-// (16 KiB) next to the basis tile, and every 128x96x16 MMA re-reads 7 KiB of operands in its 48 cycles.  This kernel is
-// built around bytes per MMA cycle instead:
-//   * the coefficient tile of a row tile (128 heads x 448 x fp16 = 112 KiB) is loaded ONCE and stays resident in shared
-//     memory while the CTA sweeps its range of vertex tiles (A-stationary); only the basis streams (TMA ring);
-//   * vertex tiles are 192 columns (64 vertices) wide: 10 KiB of operand reads per 96-cycle MMA instead of 7 KiB per 48;
-//   * CTA pairs (cta_group::2, kPair): the pair shares one 192-column basis tile, each CTA loading and holding half of it,
-//     so basis bytes through each SM's shared memory halve again (M = 256 heads per pair);
-//   * one tensor-core product per MAC (fp16 operands, 11-bit mantissa like TF32; the power-of-two pre-scaled basis keeps
-//     every operand normal).  Measured error of the vertices against the fp64 reference: relL2 1.5e-5, inside the 1e-4
-//     contract; the 3-product hi/lo mode (2e-7) remains available as DAD3D_BLEND_HILO through the tile engine.
-// Roles (320 threads): warp 0 TMA producer, warp 1 MMA issuer (one elected lane), warps 2..9 epilogue.  Two TMEM accumulator
-// buffers (2 x 192 columns): the epilogue of tile i overlaps the MMAs of tile i+1.  Epilogue warp w owns TMEM lanes 32*(w%4)..
-// (= 32 heads) and one half of the tile's columns (96 columns = 32 vertices = 4 passes of 8 vertices); the two warps of a lane
-// quarter SWAP halves every tile.  Per pass: TMEM -> registers (the next pass's load is issued before this pass's stores) ->
-// skinning with packed fp32 FMAs (fma.rn.f32x2: the basis rows of a tile are regrouped per vertex pair as x x' y y' z z', so
-// accumulator columns arrive as register pairs; 24 FFMA2 per vertex pair instead of 48 FFMA), per-pair (w_rest, w_jaw) broadcast
-// from a per-warp shared-memory table -> 256-bit global stores straight from registers.  No staging buffer, no shuffles.
+// Compared with the generic tile engine (tile_gemm.cuh, still used by the strict hi/lo mode): one tensor-core product per MAC
+// (fp16 operands, 11-bit mantissa like TF32; the power-of-two pre-scaled basis keeps every operand normal; relL2 of the
+// vertices against the fp64 reference ~1.5e-5, inside the 1e-4 contract), vertex tiles of 192 columns (64 vertices), and an
+// epilogue built around whole-sector stores.
+// Roles (384 threads): warp 0 TMA producer (one ring slot = one 64-wide k-block of the 128-head coefficient tile and of the
+// 192-column basis tile); warpgroups 1 and 2 consume: warpgroup w issues m64n192k16 wgmma for heads rows 64w.. into register
+// accumulators, writes them to a shared-memory accumulator tile and runs the epilogue on it.  Epilogue warp (w, i) owns rows
+// 32*(2w + i%2).. (= 32 heads) and one half of the tile's columns (96 columns = 32 vertices = 4 passes of 8 vertices); the two
+// warps of a row quarter SWAP halves every tile.  Per pass: shared memory -> registers -> skinning -> global stores straight
+// from registers.
 //
 // Stores.  Rows of the reference layout [B,5023,3] are only 4-byte aligned (pitch 60 276 B), and a store that covers part of a
-// 32-byte sector costs the L2 a read-modify-write (measured: 24 M heads/s with runs cut at arbitrary offsets, 37 M with
-// sector-aligned runs).  Each lane therefore writes ITS OWN row: it keeps the last 8 floats of the previous pass (the carry) and
-// writes the window of 24 floats that starts c floats earlier, at the previous sector boundary, as three st.global.v8.f32
-// (STG.256, one whole sector each).  c = (address of the pass's first float, in floats) mod 8 is constant along a row (every
-// pass advances by 3 sectors) and depends on the head index only through head mod 8 (8 x pitch = 0 mod 8 floats), so the
-// coefficient rows are PERMUTED (dec_phys_row / dec_head_of: physical row tile 2b+t, lane quarter wq, lane l <-> head
-// 256 b + 8 l + 4 t + wq) to give all 32 lanes of a warp the same c: the window selection is a warp-uniform switch over c with
-// compile-time register choices.  Sector boundaries that fall between two warps' column ranges: at a tile boundary the carry
-// stays in the registers of the warp that swaps from half 1 to half 0; inside a tile, half 1 recomputes the two vertex pairs in
-// front of its range from the same accumulator (+6 % arithmetic).  Partial sectors remain only at the two ends of a unit's
-// column range (row start / row end).  Measured steps: staged scalar stores 36.7 M heads/s -> STG.256 per lane 36.6 (partial
-// sectors at every warp boundary: the L2's read-modify-write dominates) -> + FFMA2 38.9 -> whole sectors everywhere 41.0.
+// 32-byte sector costs the L2 a read-modify-write.  Each lane therefore writes ITS OWN row: it keeps the last 8 floats of the
+// previous pass (the carry) and writes the window of 24 floats that starts c floats earlier, at the previous sector boundary,
+// as whole sectors.  c = (address of the pass's first float, in floats) mod 8 is constant along a row (every pass advances by
+// 3 sectors) and depends on the head index only through head mod 8 (8 x pitch = 0 mod 8 floats), so the coefficient rows are
+// PERMUTED (dec_phys_row / dec_head_of: physical row tile 2b+t, row quarter wq, lane l <-> head 256 b + 8 l + 4 t + wq) to
+// give all 32 lanes of a warp the same c: the window selection is a warp-uniform switch over c with compile-time register
+// choices.  Sector boundaries that fall between two warps' column ranges: at a tile boundary the carry stays in the registers
+// of the warp that swaps from half 1 to half 0; inside a tile, half 1 recomputes the two vertex pairs in front of its range
+// from the same accumulator (+6 % arithmetic).  Partial sectors remain only at the two ends of a unit's column range.
 #pragma once
 #include "ptx.cuh"
 
@@ -49,9 +37,11 @@ constexpr int kDecBlockM = 128;
 constexpr int kDecBlockK = 64;
 constexpr int kDecN = 192;                         // columns per vertex tile = 64 vertices
 constexpr int kDecKBlocks = 7;                     // 448 / 64
-constexpr int kDecABytes = kDecBlockM * kDecBlockK * 2;          // 16 KiB per k-block of the coefficient tile
-constexpr int kDecAResident = kDecKBlocks * kDecABytes;           // 112 KiB
-constexpr int kDecThreads = 320;
+constexpr int kDecABytes = kDecBlockM * kDecBlockK * 2;          // 16 KiB: one k-block of the coefficient tile
+constexpr int kDecStageBytes = kDecABytes + kDecN * kDecBlockK * 2;   // + 24 KiB of basis per ring slot
+constexpr int kDecAccStride = kDecN + 4;           // floats per accumulator row (= 4 mod 32: conflict-free row-per-lane reads)
+constexpr int kDecAccBytes = kDecBlockM * kDecAccStride * 4;
+constexpr int kDecThreads = 384;
 constexpr int kDecEpiWarps = 8;
 constexpr int kDecPassCols = 24;                   // 8 vertices per pass
 constexpr int kDecWarpCols = kDecN / 2;             // columns of a tile per epilogue warp (two column groups)
@@ -74,36 +64,28 @@ struct DecodeParams {
   int rows;                 // heads in this launch (coefficient rows are stored permuted: dec_phys_row; rows padded to 256)
   int nv;                   // vertices (5023)
   int n_tiles;              // ceil(3*nv / 192)
-  int m_units;              // row tiles (non-pair) or row-tile pairs (pair); always whole 256-head blocks
+  int m_units;              // row tiles (always whole 256-head blocks)
   int splits;               // each m unit is split into `splits` contiguous ranges of vertex tiles
-  int stages;               // depth of the basis ring (slots)
-  int kbs;                  // k-blocks per ring slot (1..4): one full/empty barrier round trip per slot
+  int stages;               // depth of the operand ring (slots)
   const float* xf;          // [rows][68] per-head transform records (flame_prep_kernel)
   const float* w2;          // [n_tiles * 64][2] (w_rest, w_jaw), zero-padded past nv
   float* verts3d;           // [rows][nv][3] or null
   float* proj;              // [rows][nv][pc] or null
   int pc;
   float image_size;
-  int poll;                 // 1: producer / MMA warps poll their barriers with test_wait instead of try_wait (A/B)
-  unsigned* prof;           // kProf instantiation only (DAD3D_DECODE_PROFILE): [block][10 warps][8] cycle counters
-  int debug;                // diagnostics only (DAD3D_DECODE_DEBUG): 2 = stores predicated off at run time, 3 = the epilogue only
-                            // hands the accumulator back (pure main-loop rate)
+  int poll;                 // 1: producer / consumer warps poll the ring barriers with test_wait instead of try_wait (A/B)
+  int debug;                // diagnostics only (DAD3D_DECODE_DEBUG): 2 = stores predicated off at run time, 3 = no epilogue
+                            // (pure main-loop rate)
 };
 
-template <bool kPair>
-__host__ __device__ inline int dec_b_stage_bytes() { return (kPair ? kDecN / 2 : kDecN) * kDecBlockK * 2; }
-template <bool kPair>
-__host__ inline int dec_max_stages(int kbs) {
-  const int fixed = kDecAResident + kDecEpiWarps * kDecWtabBytes + 1024 + 512;
-  int s = (kDecSmemLimit - fixed) / (kbs * dec_b_stage_bytes<kPair>());
+__host__ inline int dec_fixed_smem_bytes() { return kDecAccBytes + kDecEpiWarps * kDecWtabBytes + 1024 + 512; }
+__host__ inline int dec_max_stages() {
+  const int s = (kDecSmemLimit - dec_fixed_smem_bytes()) / kDecStageBytes;
   return s > 8 ? 8 : s;
 }
-template <bool kPair>
-__host__ inline int dec_smem_bytes(int stages, int kbs) {
-  return kDecAResident + stages * kbs * dec_b_stage_bytes<kPair>() + kDecEpiWarps * kDecWtabBytes + 1024 + 512;
-}
+__host__ inline int dec_smem_bytes(int stages) { return stages * kDecStageBytes + dec_fixed_smem_bytes(); }
 
-// unit u of this CTA (pair): row tile (pair) m, vertex tiles [n0, n1)
+// unit u of this CTA: row tile m, vertex tiles [n0, n1)
 __device__ __forceinline__ bool dec_unit_at(const DecodeParams& p, int group, int n_groups, int i, int* m, int* n0, int* n1) {
   const int u = group + i * n_groups;
   if (u >= p.m_units * p.splits) return false;
@@ -124,7 +106,7 @@ __device__ __forceinline__ void dec_store_c(float* __restrict__ dst, const float
 #define DEC_EXT(e) ((e) < 8 ? carry[(e) < 8 ? (e) : 0] : x[(e) >= 8 ? (e) - 8 : 0])
   float* w = dst - C;
   if (C == 0 || !head) {
-    ptx::st_global_v8(w, DEC_EXT(8 - C), DEC_EXT(9 - C), DEC_EXT(10 - C), DEC_EXT(11 - C), DEC_EXT(12 - C), DEC_EXT(13 - C),
+    ptx::st_global_8f(w, DEC_EXT(8 - C), DEC_EXT(9 - C), DEC_EXT(10 - C), DEC_EXT(11 - C), DEC_EXT(12 - C), DEC_EXT(13 - C),
                       DEC_EXT(14 - C), DEC_EXT(15 - C));
   } else {
 #pragma unroll
@@ -132,7 +114,7 @@ __device__ __forceinline__ void dec_store_c(float* __restrict__ dst, const float
   }
 #pragma unroll
   for (int k = 1; k < RUN / 8; ++k)
-    ptx::st_global_v8(w + 8 * k, DEC_EXT(8 - C + 8 * k), DEC_EXT(9 - C + 8 * k), DEC_EXT(10 - C + 8 * k), DEC_EXT(11 - C + 8 * k),
+    ptx::st_global_8f(w + 8 * k, DEC_EXT(8 - C + 8 * k), DEC_EXT(9 - C + 8 * k), DEC_EXT(10 - C + 8 * k), DEC_EXT(11 - C + 8 * k),
                       DEC_EXT(12 - C + 8 * k), DEC_EXT(13 - C + 8 * k), DEC_EXT(14 - C + 8 * k), DEC_EXT(15 - C + 8 * k));
   if (C > 0 && tail) {
 #pragma unroll
@@ -173,38 +155,25 @@ __device__ __forceinline__ void dec_wait(uint64_t* bar, uint32_t parity, int pol
   else ptx::mbar_wait(bar, parity);
 }
 
-// kProf: cycle accounting per warp role (clock() deltas summed over the launch), written to p.prof at the end:
-//   producer  [0] waiting for a free ring slot, [1] waiting for the resident tile to be released, [7] whole role
-//   MMA       [0] waiting for a free accumulator (epilogue back-pressure), [1] waiting for a full ring slot (feed starvation),
-//             [2] waiting for the coefficient tile, [6] tiles, [7] whole role
-//   epilogue  [0] waiting for a full accumulator, [1] TMEM loads, [2] skinning math, [3] staging + stores, [6] tiles, [7] whole role
-// kProj: the projected output is requested too (its carry and constants cost ~12 registers: own instantiation)
-template <bool kPair, bool kProf = false, bool kProj = true>
-__global__ void __launch_bounds__(kDecThreads, 1)   // registers are allocated per 4 warps: 320 threads count as 384 -> 168 / thread
+// kProj: the projected output is requested too (its carry and constants cost registers: own instantiation)
+template <bool kProj = true>
+__global__ void __launch_bounds__(kDecThreads, 1)
 flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficients [rows, 448] fp16, box 64 x 128
-                    const __grid_constant__ CUtensorMap map_b,     // basis [npad, 448] fp16, box 64 x (192 | 96)
+                    const __grid_constant__ CUtensorMap map_b,     // basis [npad, 448] fp16, box 64 x 192
                     const DecodeParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr int kBBlock = (kPair ? kDecN / 2 : kDecN) * kDecBlockK * 2;   // one k-block of (my half of) a basis tile
-  const int kBStage = p.kbs * kBBlock;                             // one ring slot = p.kbs k-blocks
-  uint8_t* smem_a = smem;                                          // [7][16 KiB] resident coefficient tile
-  uint8_t* smem_b = smem + kDecAResident;                          // [stages][kBStage]
-  uint8_t* wtab_all = smem_b + p.stages * kBStage;                 // [8][512 B] per-warp (w_rest, w_jaw) table of the current tile
+  uint8_t* ring = smem;                                            // [stages][A 16 KiB | B 24 KiB]
+  float* acc_smem = reinterpret_cast<float*>(smem + p.stages * kDecStageBytes);   // [128][kDecAccStride]
+  uint8_t* wtab_all = smem + p.stages * kDecStageBytes + kDecAccBytes;            // [8][320 B] per-warp (w_rest, w_jaw) table
   uint64_t* bars = reinterpret_cast<uint64_t*>(wtab_all + kDecEpiWarps * kDecWtabBytes);
-  uint64_t* full_bar = bars;                  // [8]  basis ring
+  uint64_t* full_bar = bars;                  // [8]
   uint64_t* empty_bar = bars + 8;             // [8]
-  uint64_t* afull_bar = bars + 16;            // [7]  one per k-block of the resident coefficient tile
-  uint64_t* aempty_bar = bars + 23;           // [1]  all MMAs of the unit have read it
-  uint64_t* tfull_bar = bars + 24;            // [2]
-  uint64_t* tempty_bar = bars + 26;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 28);
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int crank = kPair ? static_cast<int>(ptx::cluster_ctarank()) : 0;
-  const int group = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int n_groups = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int group = static_cast<int>(blockIdx.x);
+  const int n_groups = static_cast<int>(gridDim.x);
 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tmap(&map_a);
@@ -213,168 +182,49 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < 8; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int k = 0; k < kDecKBlocks; ++k) ptx::mbar_init(&afull_bar[k], 1);
-    ptx::mbar_init(aempty_bar, 1);
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&tfull_bar[b], 1);
-      ptx::mbar_init(&tempty_bar[b], (kPair ? 2 : 1) * kDecEpiWarps);   // one arrive per epilogue warp (pair: both CTAs')
+      ptx::mbar_init(&empty_bar[s], 2);          // one arrive per consumer warpgroup
     }
     ptx::fence_mbar_init();
   }
-  if (warp == 0) {
-    if constexpr (kPair) { ptx::tmem_alloc_2sm(tmem_slot, 512); ptx::tmem_relinquish_2sm(); }
-    else { ptx::tmem_alloc(tmem_slot, 512); ptx::tmem_relinquish(); }
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if constexpr (kPair) ptx::cluster_sync_all();     // the peer's barriers exist before anyone signals them
   ptx::grid_dep_launch();
   ptx::grid_dep_wait();
 
   if (warp == 0) {
     // ===================================================== TMA producer (whole warp walks the schedule, one lane issues)
     int stage = 0;
-    uint32_t phase = 0, aphase = 0;
+    uint32_t phase = 0;
     int m, n0, n1;
-    unsigned pc0 = 0, pc1 = 0, pt0 = 0, pstart = 0;
-    if constexpr (kProf) pstart = clock();
     for (int ui = 0; dec_unit_at(p, group, n_groups, ui, &m, &n0, &n1); ++ui) {
-      // the resident coefficient tile may be overwritten once every MMA of the previous unit has read it
-      if constexpr (kProf) pt0 = clock();
-      dec_wait(aempty_bar, aphase ^ 1u, p.poll);
-      if constexpr (kProf) pc1 += clock() - pt0;
-      const int row0 = (kPair ? 2 * m + crank : m) * kDecBlockM;
-      if (ptx::elect_one_sync()) {
-        for (int kb = 0; kb < kDecKBlocks; ++kb) {
-          if constexpr (kPair) {
-            const uint32_t lead = ptx::mapa_u32(&afull_bar[kb], 0);
-            if (crank == 0) ptx::mbar_expect_tx(&afull_bar[kb], 2 * kDecABytes);
-            ptx::tma_load_2d_2sm(smem_a + kb * kDecABytes, &map_a, lead, kb * kDecBlockK, row0);
-          } else {
-            ptx::mbar_expect_tx(&afull_bar[kb], kDecABytes);
-            ptx::tma_load_2d(smem_a + kb * kDecABytes, &map_a, &afull_bar[kb], kb * kDecBlockK, row0);
-          }
-        }
-      }
-      __syncwarp();
-      aphase ^= 1u;
       for (int n = n0; n < n1; ++n) {
-        for (int kb0 = 0; kb0 < kDecKBlocks; kb0 += p.kbs) {
-          const int nk = min(p.kbs, kDecKBlocks - kb0);
-          if constexpr (kProf) pt0 = clock();
+        for (int kb = 0; kb < kDecKBlocks; ++kb) {
           dec_wait(&empty_bar[stage], phase ^ 1u, p.poll);
-          if constexpr (kProf) pc0 += clock() - pt0;
           if (ptx::elect_one_sync()) {
-            if constexpr (kPair) {
-              const uint32_t lead = ptx::mapa_u32(&full_bar[stage], 0);
-              if (crank == 0) ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(2 * nk * kBBlock));
-              for (int j = 0; j < nk; ++j)
-                ptx::tma_load_2d_2sm(smem_b + stage * kBStage + j * kBBlock, &map_b, lead, (kb0 + j) * kDecBlockK,
-                                     n * kDecN + crank * (kDecN / 2));
-            } else {
-              ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(nk * kBBlock));
-              for (int j = 0; j < nk; ++j)
-                ptx::tma_load_2d(smem_b + stage * kBStage + j * kBBlock, &map_b, &full_bar[stage], (kb0 + j) * kDecBlockK,
-                                 n * kDecN);
-            }
+            uint8_t* st = ring + stage * kDecStageBytes;
+            ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(kDecStageBytes));
+            ptx::tma_load_2d(st, &map_a, &full_bar[stage], kb * kDecBlockK, m * kDecBlockM);
+            ptx::tma_load_2d(st + kDecABytes, &map_b, &full_bar[stage], kb * kDecBlockK, n * kDecN);
           }
           __syncwarp();
           if (++stage == p.stages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-    if constexpr (kProf) {
-      if (lane == 0) {
-        unsigned* o = p.prof + (static_cast<size_t>(blockIdx.x) * 10 + 0) * 8;
-        o[0] = pc0; o[1] = pc1; o[7] = clock() - pstart;
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (!kPair || crank == 0) {
-      const uint32_t idesc = ptx::make_idesc_f16(0u, kPair ? 2 * kDecBlockM : kDecBlockM, kDecN);
-      int stage = 0;
-      uint32_t phase = 0, aphase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int m, n0, n1;
-      unsigned mc0 = 0, mc1 = 0, mc2 = 0, mt0 = 0, mtiles = 0, mstart = 0, mu0 = 0, mu1 = 0, mu2 = 0;
-      if constexpr (kProf) mstart = clock();
-      for (int ui = 0; dec_unit_at(p, group, n_groups, ui, &m, &n0, &n1); ++ui) {
-        for (int n = n0; n < n1; ++n) {
-          if constexpr (kProf) mt0 = clock();
-          dec_wait(&tempty_bar[acc], acc_phase ^ 1u, p.poll);
-          if constexpr (kProf) { mc0 += clock() - mt0; ++mtiles; }
-          ptx::tc_fence_after();
-          const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * kDecN);
-          for (int kb0 = 0; kb0 < kDecKBlocks; kb0 += p.kbs) {
-            const int nk = min(p.kbs, kDecKBlocks - kb0);
-            if constexpr (kProf) mt0 = clock();
-            if (n == n0)                                             // first sweep over the freshly loaded coefficient tile
-              for (int j = 0; j < nk; ++j) dec_wait(&afull_bar[kb0 + j], aphase, p.poll);
-            if constexpr (kProf) { const unsigned t = clock(); mc2 += t - mt0; mt0 = t; }
-            dec_wait(&full_bar[stage], phase, p.poll);
-            if constexpr (kProf) mc1 += clock() - mt0;
-            ptx::tc_fence_after();
-            const uint32_t sa0 = ptx::smem_u32(smem_a + kb0 * kDecABytes);
-            const uint32_t sb0 = ptx::smem_u32(smem_b + stage * kBStage);
-            const bool last = kb0 + nk == kDecKBlocks;
-            if (ptx::elect_one_sync()) {
-              for (int j = 0; j < nk; ++j) {
-                const uint64_t adesc = ptx::make_kmajor_sw128_desc(sa0 + j * kDecABytes);
-                const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb0 + j * kBBlock);
+  } else if (warp >= 4) {
+    // ===================================================== consumer warpgroups: wgmma main loop + skinning epilogue
+    const int wg = (warp - 4) >> 2;                // tile rows 64*wg ..
+    const int wl = warp & 3;
+    const int wq = 2 * wg + (wl & 1);              // row quarter of the epilogue: rows 32*wq + lane
+    const int grp = wl >> 1;                       // column half of even tiles (the halves swap every tile)
+    const bool signaller = wl == 0 && lane == 0;
+    float4* wtab = reinterpret_cast<float4*>(wtab_all + (warp - 4) * kDecWtabBytes);
+    const float* arow = acc_smem + (wq * 32 + lane) * kDecAccStride;   // this thread's accumulator row
+    float acc[kDecN / 2];
 #pragma unroll
-                for (int k = 0; k < kDecBlockK / 16; ++k) {
-                  const uint32_t accum = (kb0 + j > 0 || k > 0) ? 1u : 0u;
-                  if constexpr (kPair) ptx::umma_f16_2sm(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc, accum);
-                  else ptx::umma_f16(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc, accum);
-                }
-              }
-              if constexpr (kPair) ptx::umma_commit_2sm_mc(&empty_bar[stage], 3);
-              else ptx::umma_commit(&empty_bar[stage]);
-              if (last) {
-                if constexpr (kPair) ptx::umma_commit_2sm_mc(&tfull_bar[acc], 3);
-                else ptx::umma_commit(&tfull_bar[acc]);
-                if (n == n1 - 1) {                                   // the unit's last MMAs: the coefficient tile is free after them
-                  if constexpr (kPair) ptx::umma_commit_2sm_mc(aempty_bar, 3);
-                  else ptx::umma_commit(aempty_bar);
-                }
-              }
-            }
-            __syncwarp();
-            if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-          }
-          acc ^= 1;
-          if (acc == 0) acc_phase ^= 1u;
-        }
-        aphase ^= 1u;
-        if constexpr (kProf) {                       // coefficient wait of the first three units separately
-          if (ui == 0) mu0 = mc2;
-          if (ui == 1) mu1 = mc2 - mu0;
-          if (ui == 2) mu2 = mc2 - mu0 - mu1;
-        }
-      }
-      if constexpr (kProf) {
-        if (lane == 0) {
-          unsigned* o = p.prof + (static_cast<size_t>(blockIdx.x) * 10 + 1) * 8;
-          o[0] = mc0; o[1] = mc1; o[2] = mc2; o[3] = mu0; o[4] = mu1; o[5] = mu2; o[6] = mtiles; o[7] = clock() - mstart;
-        }
-      }
-    }
-  } else {
-    // ===================================================== epilogue warps
-    const int wq = warp & 3;                       // TMEM lane quarter
-    const int grp = (warp - 2) >> 2;               // epilogue group = accumulator buffer: tiles with (tile counter & 1) == grp
-    float4* wtab = reinterpret_cast<float4*>(wtab_all + (warp - 2) * kDecWtabBytes);
-    const uint32_t tempty_remote0 = kPair ? ptx::mapa_u32(&tempty_bar[0], 0) : 0u;
-    const uint32_t tempty_remote1 = kPair ? ptx::mapa_u32(&tempty_bar[1], 0) : 0u;
-    int acc = 0;                                   // accumulator buffer of the current tile: alternates per tile, across units too
-    uint32_t acc_phase = 0;
-    float2 R2[12], J2[12], c2x, c2y, c2z;          // per-head transforms and offset, both halves equal (operands of the packed FMAs)
+    for (int i = 0; i < kDecN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    float R[12], J[12], c0x, c0y, c0z;             // per-head transforms (rest, jaw) and offset
     float sc = 1.f, tx = 0.f, ty = 0.f;
     int m, n0, n1;
     const int nv3 = p.nv * 3;
@@ -383,92 +233,106 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
     float vcar[8], qcar[8];                        // this row's last 8 floats of the previous pass (the carry), per output
 #pragma unroll
     for (int j = 0; j < 8; ++j) vcar[j] = qcar[j] = 0.f;
-    unsigned ec0 = 0, ec1 = 0, ec2 = 0, ec3 = 0, et0 = 0, etiles = 0, estart = 0;
-    if constexpr (kProf) estart = clock();
-    const uint32_t t_wq = tmem_base + (static_cast<uint32_t>(wq * 32) << 16);
     for (int ui = 0; dec_unit_at(p, group, n_groups, ui, &m, &n0, &n1); ++ui) {
-      const int head = dec_head_of(kPair ? 2 * m + crank : m, wq, lane);
+      const int head = dec_head_of(m, wq, lane);
       const bool row_ok = head < p.rows && p.debug != 2;
-      {   // per-head transforms -> registers, once per unit (rows past the batch read the last valid record; never stored)
+      auto load_transforms = [&]() {   // rows past the batch read the last valid record; never stored
         const int h = min(head, p.rows - 1);
         const float4* src = reinterpret_cast<const float4*>(p.xf + static_cast<size_t>(h) * kDecXfFloats);
 #pragma unroll
         for (int q = 0; q < 3; ++q) {
           const float4 a = __ldg(&src[q]);           // joint 0 (rest)
           const float4 b = __ldg(&src[6 + q]);       // joint 2 (jaw)
-          R2[4 * q] = make_float2(a.x, a.x); R2[4 * q + 1] = make_float2(a.y, a.y);
-          R2[4 * q + 2] = make_float2(a.z, a.z); R2[4 * q + 3] = make_float2(a.w, a.w);
-          J2[4 * q] = make_float2(b.x, b.x); J2[4 * q + 1] = make_float2(b.y, b.y);
-          J2[4 * q + 2] = make_float2(b.z, b.z); J2[4 * q + 3] = make_float2(b.w, b.w);
+          R[4 * q] = a.x; R[4 * q + 1] = a.y; R[4 * q + 2] = a.z; R[4 * q + 3] = a.w;
+          J[4 * q] = b.x; J[4 * q + 1] = b.y; J[4 * q + 2] = b.z; J[4 * q + 3] = b.w;
         }
         const float4 u = __ldg(&src[15]);
         const float4 w = __ldg(&src[16]);
-        c2x = make_float2(u.x, u.x); c2y = make_float2(u.y, u.y); c2z = make_float2(u.z, u.z);
+        c0x = u.x; c0y = u.y; c0z = u.z;
         sc = u.w; tx = w.x; ty = w.y;
-      }
+      };
       float* const v_row = p.verts3d ? p.verts3d + static_cast<size_t>(min(head, p.rows - 1)) * nv3 : nullptr;
       float* const q_row = (kProj && p.proj) ? p.proj + static_cast<size_t>(min(head, p.rows - 1)) * p.nv * pc : nullptr;
       // sector phase of the row (floats mod 8): the same for all lanes of the warp (heads = const mod 8), constant along the row
       const unsigned c_v = __shfl_sync(0xffffffffu, static_cast<unsigned>((reinterpret_cast<uintptr_t>(v_row) >> 2) & 7u), 0);
       const unsigned c_q = __shfl_sync(0xffffffffu, static_cast<unsigned>((reinterpret_cast<uintptr_t>(q_row) >> 2) & 7u), 0);
-      for (int n = n0; n < n1; ++n, acc ^= 1, acc_phase ^= (acc == 0 ? 1u : 0u)) {
-        // Column half of this warp: the two warps of a lane quarter SWAP halves every tile, so the warp that ends tile n (half 1)
+      for (int n = n0; n < n1; ++n) {
+        // ---- main loop: this warpgroup's 64 coefficient rows x the 192 basis columns of tile n, K = 448
+        int pend = -1;
+        for (int kb = 0; kb < kDecKBlocks; ++kb) {
+          dec_wait(&full_bar[stage], phase, p.poll);
+          const uint32_t sa = ptx::smem_u32(ring + stage * kDecStageBytes) + static_cast<uint32_t>(wg * 64 * kDecBlockK * 2);
+          const uint32_t sb = ptx::smem_u32(ring + stage * kDecStageBytes + kDecABytes);
+          const uint64_t adesc = ptx::make_kmajor_sw128_desc(sa);
+          const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb);
+          ptx::wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kDecBlockK / 16; ++k)
+            ptx::wgmma_m64k16<kDecN, 0>(acc, adesc + 2u * k, bdesc + 2u * k, (kb > 0 || k > 0) ? 1u : 0u);
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();                  // the previous k-block's group is complete: its slot may be refilled
+          if (pend >= 0 && signaller) ptx::mbar_arrive(&empty_bar[pend]);
+          pend = stage;
+          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+        }
+        ptx::wgmma_wait<0>();
+        if (signaller) ptx::mbar_arrive(&empty_bar[pend]);
+        ptx::reg_fence(acc);
+        // ---- accumulator (this warpgroup's 64 rows) -> shared memory; each epilogue lane then reads its own row
+        ptx::bar_sync(1 + wg, 128);              // the previous tile's rows have been read by every warp of the warpgroup
+        {
+          const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+#pragma unroll
+          for (int j = 0; j < kDecN / 8; ++j) {
+            const int col = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc_smem + r0 * kDecAccStride + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(acc_smem + (r0 + 8) * kDecAccStride + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        }
+        ptx::bar_sync(1 + wg, 128);
+        if (p.debug == 3) continue;
+        load_transforms();                       // per tile (L1-resident): not live across the main loop's accumulators
+        // Column half of this warp: the two warps of a row quarter SWAP halves every tile, so the warp that ends tile n (half 1)
         // begins tile n+1 (half 0) and the carry across the tile boundary stays in its registers.  Half 1 begins inside the tile:
         // it recomputes the two vertex pairs in front of its range from the same accumulator (12 more columns, +6 % arithmetic)
         // to get its carry.  With that every sector inside a unit's column range is written whole, by one lane.
         const int half = grp ^ (n & 1);
-        const uint32_t t_lane = t_wq + static_cast<uint32_t>(acc * kDecN + half * kDecWarpCols);
-        const uint32_t tempty_remote = acc ? tempty_remote1 : tempty_remote0;
+        const float* a_lane = arow + half * kDecWarpCols;
         // (w_rest, w_jaw) per vertex pair -- pairs [14 half, 14 half + 18) of the tile: entries 0, 1 are the two pairs in front of
-        // half 1 (unused by half 0), entries 2.. the warp's own 16.  The L2 latency hides behind the wait for the accumulator.
+        // half 1 (unused by half 0), entries 2.. the warp's own 16.
         const float4 wv = __ldg(reinterpret_cast<const float4*>(p.w2) + static_cast<size_t>(n) * (kDecN / 6) +
                                 min(max(16 * half - 2 + lane, 0), kDecN / 6 - 1));
         const int col_t = n * kDecN + half * kDecWarpCols;   // first float of the warp's column range within a row
-        if constexpr (kProf) et0 = clock();
-        ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-        if constexpr (kProf) { ec0 += clock() - et0; ++etiles; }
-        ptx::tc_fence_after();
-        if (p.debug == 3) {
-          ptx::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (kPair) ptx::mbar_arrive_cluster_relaxed(tempty_remote);
-            else ptx::mbar_arrive_relaxed(&tempty_bar[acc]);
-          }
-          continue;
-        }
-        // Skinning of one vertex pair with packed fp32 FMAs (fma.rn.f32x2): the basis rows of a tile are regrouped per vertex
-        // pair as (x x' y y' z z'), so the accumulator columns arrive as ready-made register pairs; the per-head constants are
-        // held duplicated.  24 FFMA2 per vertex pair instead of 48 FFMA -- the epilogue is issue-bound.
+        // Skinning of one vertex pair: the basis rows of a tile are regrouped per vertex pair as (x x' y y' z z'), so the
+        // accumulator columns of the two vertices are interleaved.
         auto skin_pair = [&](const float* a6, const float4& w4, float* o6) {
-          const float2 wr = make_float2(w4.x, w4.y), wj = make_float2(w4.z, w4.w);   // (w_rest v, w_rest v'), (w_jaw v, w_jaw v')
-          const float2 px = make_float2(a6[0], a6[1]), py = make_float2(a6[2], a6[3]), pz = make_float2(a6[4], a6[5]);
-          const float2 rx = __ffma2_rn(R2[0], px, __ffma2_rn(R2[1], py, __ffma2_rn(R2[2], pz, R2[3])));
-          const float2 ry = __ffma2_rn(R2[4], px, __ffma2_rn(R2[5], py, __ffma2_rn(R2[6], pz, R2[7])));
-          const float2 rz = __ffma2_rn(R2[8], px, __ffma2_rn(R2[9], py, __ffma2_rn(R2[10], pz, R2[11])));
-          const float2 jx = __ffma2_rn(J2[0], px, __ffma2_rn(J2[1], py, __ffma2_rn(J2[2], pz, J2[3])));
-          const float2 jy = __ffma2_rn(J2[4], px, __ffma2_rn(J2[5], py, __ffma2_rn(J2[6], pz, J2[7])));
-          const float2 jz = __ffma2_rn(J2[8], px, __ffma2_rn(J2[9], py, __ffma2_rn(J2[10], pz, J2[11])));
-          const float2 ox = __ffma2_rn(wj, jx, __ffma2_rn(wr, rx, c2x));
-          const float2 oy = __ffma2_rn(wj, jy, __ffma2_rn(wr, ry, c2y));
-          const float2 oz = __ffma2_rn(wj, jz, __ffma2_rn(wr, rz, c2z));
-          o6[0] = ox.x; o6[1] = oy.x; o6[2] = oz.x;
-          o6[3] = ox.y; o6[4] = oy.y; o6[5] = oz.y;
+#pragma unroll
+          for (int v = 0; v < 2; ++v) {
+            const float wr = v ? w4.y : w4.x, wj = v ? w4.w : w4.z;
+            const float px = a6[v], py = a6[2 + v], pz = a6[4 + v];
+            const float rx = fmaf(R[0], px, fmaf(R[1], py, fmaf(R[2], pz, R[3])));
+            const float ry = fmaf(R[4], px, fmaf(R[5], py, fmaf(R[6], pz, R[7])));
+            const float rz = fmaf(R[8], px, fmaf(R[9], py, fmaf(R[10], pz, R[11])));
+            const float jx = fmaf(J[0], px, fmaf(J[1], py, fmaf(J[2], pz, J[3])));
+            const float jy = fmaf(J[4], px, fmaf(J[5], py, fmaf(J[6], pz, J[7])));
+            const float jz = fmaf(J[8], px, fmaf(J[9], py, fmaf(J[10], pz, J[11])));
+            o6[3 * v] = fmaf(wj, jx, fmaf(wr, rx, c0x));
+            o6[3 * v + 1] = fmaf(wj, jy, fmaf(wr, ry, c0y));
+            o6[3 * v + 2] = fmaf(wj, jz, fmaf(wr, rz, c0z));
+          }
         };
-        // (Issuing the load of pass q+1 before the arithmetic of pass q, into a second register buffer, was measured: the wait for
-        // the columns shrinks from ~400 to ~100 cycles per pass but the time reappears in the stores -- the store path is the
-        // bottleneck -- and the kernel gets 4 % slower.)
-        float xa[24];
-        if constexpr (kProf) et0 = clock();
-        float xb[16];
-        if (half) ptx::tmem_ld_32x32b_x16_f(t_lane - 16, xb);      // the 12 columns in front of half 1 (4 more ride along)
-        ptx::tmem_ld_32x32b_x16_f(t_lane, xa);
-        ptx::tmem_ld_32x32b_x8_f(t_lane + 16, xa + 16);
+        auto load_cols = [&](const float* src, float* dst, int n4) {
+          for (int j = 0; j < n4; ++j) {
+            const float4 v = *reinterpret_cast<const float4*>(src + 4 * j);
+            dst[4 * j] = v.x; dst[4 * j + 1] = v.y; dst[4 * j + 2] = v.z; dst[4 * j + 3] = v.w;
+          }
+        };
         __syncwarp();                                // the previous tile's table reads are done
         if (lane < 18) wtab[lane] = wv;
         __syncwarp();
         if (half) {                                  // carry of half 1: the last 8 floats in front of column 96 of the tile
-          ptx::tmem_ld_wait_16(xb);
+          float xb[16];
+          load_cols(a_lane - 16, xb, 4);             // the 12 columns in front of half 1 (4 more ride along)
           float xpre[12];
           skin_pair(xb + 4, wtab[0], xpre);
           skin_pair(xb + 10, wtab[1], xpre + 6);
@@ -492,23 +356,11 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
         }
 #pragma unroll 1
         for (int q = 0; q < kDecPasses; ++q) {       // 4 passes of 8 vertices (24 accumulator columns)
-          ptx::tmem_ld_wait_24(xa);
-          if constexpr (kProf) { const unsigned t = clock(); ec1 += t - et0; et0 = t; }
+          float xa[24];
+          load_cols(a_lane + q * kDecPassCols, xa, 6);
           float x[24];
 #pragma unroll
           for (int i = 0; i < 4; ++i) skin_pair(xa + 6 * i, wtab[2 + 4 * q + i], x + 6 * i);
-          if (q + 1 < kDecPasses) {                  // next pass's accumulator columns: in flight behind this pass's stores
-            ptx::tmem_ld_32x32b_x16_f(t_lane + (q + 1) * kDecPassCols, xa);
-            ptx::tmem_ld_32x32b_x8_f(t_lane + (q + 1) * kDecPassCols + 16, xa + 16);
-          } else {                                   // the warp's share of the accumulator has been read: hand the buffer back
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (kPair) ptx::mbar_arrive_cluster_relaxed(tempty_remote);
-              else ptx::mbar_arrive_relaxed(&tempty_bar[acc]);
-            }
-          }
-          if constexpr (kProf) { const unsigned t = clock(); ec2 += t - et0; et0 = t; }
           const int col0 = col_t + q * kDecPassCols;
           const int ncols = nv3 - col0;              // valid floats from this pass's first one to the end of the row
           if (ncols > 0) {
@@ -556,26 +408,11 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
               }
             }
           }
-          if constexpr (kProf) { ec3 += clock() - et0; et0 = clock(); }
         }
       }
     }
-    if constexpr (kProf) {
-      if (lane == 0) {
-        unsigned* o = p.prof + (static_cast<size_t>(blockIdx.x) * 10 + warp) * 8;
-        o[0] = ec0; o[1] = ec1; o[2] = ec2; o[3] = ec3; o[6] = etiles; o[7] = clock() - estart;
-      }
-    }
   }
-
-  ptx::tc_fence_before();
   __syncthreads();
-  if constexpr (kPair) ptx::cluster_sync_all();      // nobody leaves while the peer may still signal my barriers
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    if constexpr (kPair) ptx::tmem_dealloc_2sm(tmem_base, 512);
-    else ptx::tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace dad3d

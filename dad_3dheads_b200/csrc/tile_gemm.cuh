@@ -1,6 +1,6 @@
-// Persistent, warp-specialised tcgen05 tile engine for sm_100a.
+// Persistent, warp-specialised wgmma tile engine for sm_90a.
 //
-//   D[128 x block_n] (fp32, TMEM)  =  sum over k-blocks, over (a_piece, b_piece) pairs   A_piece[128 x 64] * B_piece[block_n x 64]^T
+//   D[128 x block_n] (fp32)  =  sum over k-blocks, over (a_piece, b_piece) pairs   A_piece[128 x 64] * B_piece[block_n x 64]^T
 //
 // One kernel serves every dense contraction on the hot path:
 //   * the FLAME blend-shape product  (plain GEMM: rows = heads, K = betas | pose features, N = 3*5023 coordinates), and
@@ -8,27 +8,27 @@
 //     filter taps x 64-channel blocks; the A tile for a tap is a TMA box at shifted coordinates, zero-filled outside the
 //     image, so padding costs nothing and no im2col buffer exists).
 //
-// Operands are 16-bit (fp16 or bf16, chosen in the instruction descriptor).  fp32-class accuracy comes from splitting each
-// fp32 operand into "pieces" (x = p0 + p1 [+ p2], each piece 16-bit) stored as separate planes; the MMA list names which
-// (A piece, B piece) products are accumulated (1 product = plain 16-bit GEMM, 3 = hi*hi + hi*lo + lo*hi, 6 = three-way).
+// Operands are 16-bit (fp16 or bf16).  fp32-class accuracy comes from splitting each fp32 operand into "pieces"
+// (x = p0 + p1 [+ p2], each piece 16-bit) stored as separate planes; the MMA list names which (A piece, B piece) products
+// are accumulated (1 product = plain 16-bit GEMM, 3 = hi*hi + hi*lo + lo*hi, 6 = three-way).
 //
 // Accumulator classes: the tensor core adds into its fp32 accumulator with truncation, so every MMA issued against a
 // LARGE accumulator costs up to one ulp of systematic (round-toward-zero) error.  With n_acc = 2 the dominant hi*hi
-// products go to accumulator 0 and all the small correction products to accumulator 1; the epilogue adds the two in
-// fp32 with round-to-nearest.  That cuts the number of truncating steps on the large accumulator by n_mma (6x / 3x).
+// products go to accumulator 0 and all the small correction products to accumulator 1; the two are added in fp32 with
+// round-to-nearest when the tile is written out.  That cuts the number of truncating steps on the large accumulator by
+// n_mma (6x / 3x).
 //
-// Roles (320 threads): warp 0 = TMEM allocator + TMA producer, warp 1 = barrier init + MMA issuer -- both walk their schedule
-// with all 32 lanes converged and one elect.sync lane issues the TMA / tcgen05 instructions (operands stay in uniform
-// registers; gating the warps on lane == 0 instead costs an ELECT..BRA.U.ANY loop per instruction, ~140 cycles per MMA);
-// warps 2..9 = epilogue: warp w owns TMEM lanes 32*(w%4).. (accumulator rows) and column group (w-2)/4 (half of the
-// tile's columns), i.e. two epilogue warps per SM sub-partition so their dependent-issue stalls overlap.
-// Pipelines: smem ring (full/empty mbarriers) between TMA and MMA; two TMEM accumulator buffers (tmem_full/tmem_empty)
-// between MMA and epilogue, so the epilogue of tile i overlaps the main loop of tile i+1.  Each epilogue warp owns a
-// 4 KiB shared-memory staging area (two 2 KiB store tiles used alternately) from which it issues TMA stores of its
-// 32 rows x 32 channels.
+// Roles (384 threads = 3 warpgroups): warp 0 = TMA producer (the whole warp walks the schedule, one elect.sync lane issues;
+// warps 1..3 only give their registers back); warpgroups 1 and 2 = consumers: warpgroup w issues the wgmma for tile rows
+// 64w .. 64w+63 (register accumulators), then writes them to a shared-memory accumulator tile and runs the epilogue on
+// them, each thread owning one accumulator row (warp (w, i): rows 32*(2w + i%2) + lane, column group i/2).
+// Pipeline: smem ring (full/empty mbarriers) between TMA and the consumers; a consumer releases a slot as soon as the
+// wgmma group that read it has completed, so the producer refills it while the next k-block's MMAs run and while the
+// epilogue of a tile runs.  Each epilogue warp owns a 4 KiB shared-memory staging area (two 2 KiB store tiles used
+// alternately) from which it issues TMA stores of its 32 rows x 32 channels.
 // Variants selected per launch in GemmGeom: halo (3x3 stride-1 convolutions: one halo patch per channel block feeds all nine
 // taps through shifted descriptors; separate weights ring), res_kb / res_kind (residual or second source on the K axis),
-// cl_m x cl_n multicast clusters, pair (cta_group::2, template parameter kPair).
+// cl_m x cl_n multicast clusters.
 #pragma once
 #include "ptx.cuh"
 
@@ -40,9 +40,8 @@ constexpr int kTileABytes = kBlockM * kBlockK * 2;   // 16 KiB per A piece per s
 constexpr int kMaxPieces = 3;
 constexpr int kMaxMma = 6;
 constexpr int kEpiWarps = 8;
-constexpr int kFirstEpiWarp = 2;
-constexpr int kGemmThreads = (kFirstEpiWarp + kEpiWarps) * 32;   // 320 threads
-constexpr int kTmemCols = 512;
+constexpr int kFirstEpiWarp = 4;
+constexpr int kGemmThreads = (kFirstEpiWarp + kEpiWarps) * 32;   // 384 threads
 constexpr int kStageOutBytes = 4096;              // per epilogue warp: 32 rows x 128 B
 constexpr int kGemmSmemLimit = 227 * 1024;
 // halo mode (3x3 stride-1 convolutions): output tiles of 8 x 16 pixels, input halo patch of 10 x 18 pixels per 64-channel
@@ -60,11 +59,11 @@ struct GemmGeom {
   int R, S, pad_h, pad_w;          // filter taps and padding
   int cin_blocks;                  // padded Cin / 64
   int n_tiles;                     // padded Cout / block_n
-  int block_n;                     // UMMA N: multiple of 32, 32..256
+  int block_n;                     // wgmma N: 64, 80, 96 or 128
   int nA, nB;                      // operand pieces
   int n_mma;                       // number of (a,b) piece products
   int mma_a[kMaxMma], mma_b[kMaxMma];
-  int n_acc;                       // 1 or 2 TMEM accumulators per tile (2 * n_acc * block_n <= 512 columns)
+  int n_acc;                       // 1 or 2 register accumulators per tile
   int mma_acc[kMaxMma];            // which accumulator each product goes to (see "accumulator classes" above)
   int res_kb;                      // residual-as-K-extension: after the conv's k-blocks, block_n/64 more k-blocks whose A
                                    // tiles come from the residual tensor (maps.r, at the OUTPUT pixel coordinates, the
@@ -92,11 +91,6 @@ struct GemmGeom {
                                    // ring (`stages_b` deep).  k order: channel block outer, tap inner.  A bytes per tile
                                    // drop 9 x 16 KiB -> 22.5 KiB per block and piece.
   int stages_b;                    // halo mode: depth of the B (weights) ring
-  int pair;                        // 1: CTA pair (cluster of 2, tcgen05 cta_group::2): the pair computes a 256 x block_n tile,
-                                   // CTA r owns rows 128r.. (its own A tile and accumulator) and loads rows
-                                   // [r*block_n/2, (r+1)*block_n/2) of the B tile only; the leader (rank 0) issues every
-                                   // MMA (M = 256) and owns the full / tmem-empty barriers.  Operand bytes per CTA:
-                                   // A + B/2.  Requires cl_m == cl_n == 1, block_n == 128, sched 0.
   int rowmap_n;                    // > 0: only `rowmap_n` groups of th output rows are computed; tile row index ih maps to
   unsigned char rowmap[32];        // first output row rowmap[ih] (tiles_h == rowmap_n).  Used for the heat-map head when only the
                                    // bilinear support of the FusionLayer's 64 -> 16 resampling is needed (flame_regression.py:33-41)
@@ -114,25 +108,28 @@ struct GemmMaps {
 };
 
 __host__ __device__ inline int gemm_stage_bytes(const GemmGeom& g) {
-  return g.nA * kTileABytes + g.nB * (g.block_n >> g.pair) * kBlockK * 2;
+  return g.nA * kTileABytes + g.nB * g.block_n * kBlockK * 2;
 }
 __host__ __device__ inline int gemm_halo_a_stage_bytes(const GemmGeom& g) { return g.nA * kHaloPieceBytes; }
 __host__ __device__ inline int gemm_b_stage_bytes(const GemmGeom& g) { return g.nB * g.block_n * kBlockK * 2; }
-__host__ inline int gemm_fixed_smem_bytes(int extra = 0) {
-  return kEpiWarps * kStageOutBytes + extra + 1024 /*align slack*/ + 512 /*barriers*/;
+// shared-memory accumulator tile: 128 rows of gemm_acc_stride floats, 16-byte chunks XOR-swizzled by (row & 7)
+__host__ __device__ inline int gemm_acc_stride(const GemmGeom& g) { return (g.block_n + 31) / 32 * 32; }
+__host__ __device__ inline int gemm_acc_bytes(const GemmGeom& g) { return kBlockM * gemm_acc_stride(g) * 4; }
+__host__ inline int gemm_fixed_smem_bytes(const GemmGeom& g, int extra = 0) {
+  return kEpiWarps * kStageOutBytes + gemm_acc_bytes(g) + extra + 1024 /*align slack*/ + 512 /*barriers*/;
 }
 __host__ inline int gemm_max_stages(const GemmGeom& g, int extra = 0) {
-  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(extra)) / gemm_stage_bytes(g);
+  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(g, extra)) / gemm_stage_bytes(g);
   return s > 8 ? 8 : s;
 }
 // halo mode: A ring fixed at 2 stages, the rest goes to the weights ring (0 if it does not fit)
 __host__ inline int gemm_halo_b_stages(const GemmGeom& g, int a_stages = 2) {
-  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(0) - a_stages * gemm_halo_a_stage_bytes(g)) / gemm_b_stage_bytes(g);
+  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(g) - a_stages * gemm_halo_a_stage_bytes(g)) / gemm_b_stage_bytes(g);
   return s > 8 ? 8 : s;
 }
 __host__ inline int gemm_smem_bytes(const GemmGeom& g, int extra = 0) {
-  if (g.halo) return g.stages * gemm_halo_a_stage_bytes(g) + g.stages_b * gemm_b_stage_bytes(g) + gemm_fixed_smem_bytes(extra);
-  return g.stages * gemm_stage_bytes(g) + gemm_fixed_smem_bytes(extra);
+  if (g.halo) return g.stages * gemm_halo_a_stage_bytes(g) + g.stages_b * gemm_b_stage_bytes(g) + gemm_fixed_smem_bytes(g, extra);
+  return g.stages * gemm_stage_bytes(g) + gemm_fixed_smem_bytes(g, extra);
 }
 
 struct TileCoord {
@@ -157,14 +154,7 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmGeom& g, int m_tile, 
 __device__ __forceinline__ bool tile_at(const GemmGeom& g, int i, TileCoord* tc) {
   const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
   int m, n;
-  if (g.pair) {
-    // pairs walk (row-tile pair, column tile) round-robin with the column tile fastest; a trailing odd row tile leaves the
-    // second CTA a ghost tile (zero-filled loads, clipped stores) so both CTAs run the same pipeline steps
-    const int t = static_cast<int>(blockIdx.x >> 1) + i * static_cast<int>(gridDim.x >> 1);
-    if (t >= ((m_tiles + 1) >> 1) * g.n_tiles) return false;
-    n = t % g.n_tiles;
-    m = (t / g.n_tiles) * 2 + static_cast<int>(ptx::cluster_ctarank());
-  } else if (g.sched == 0) {
+  if (g.sched == 0) {
     const int t = static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x);
     if (t >= m_tiles * g.n_tiles) return false;
     n = t % g.n_tiles;
@@ -189,21 +179,20 @@ __device__ __forceinline__ bool tile_at(const GemmGeom& g, int i, TileCoord* tc)
   return true;
 }
 
-// Everything an epilogue warp needs for one tile.
+// Everything an epilogue thread needs for one tile.
 struct EpiCtx {
   const GemmGeom* g;
   const GemmMaps* maps;
   TileCoord tc;
-  int wq;            // TMEM lane quarter of this warp (0..3): accumulator rows 32*wq .. 32*wq+31
+  int wq;            // row quarter of this warp (0..3): accumulator rows 32*wq .. 32*wq+31
   int grp;           // column group (0/1)
   int lane;
-  uint32_t t_acc;    // TMEM address of (lane quarter, accumulator buffer of this tile, accumulator class 0, column 0)
+  const float* acc;  // this thread's row of the shared-memory accumulator tile (both accumulator classes summed)
+  int swz;           // its 16-byte chunk swizzle (row & 7)
   uint8_t* stage;    // warp-private 4 KiB staging tile (1024-byte aligned)
   uint8_t* extra;    // Epi::kExtraSmemBytes of CTA-wide shared memory (epilogue-specific use)
   int prev_m_tile;   // row tile of the previous tile this CTA processed (-1 for the first)
   mutable int store_seq;   // number of TMA stores this warp has issued (epilogues alternating between two staging tiles)
-  uint64_t* tempty;  // arrive here (every epilogue thread, once) when the accumulator has been drained into registers
-  uint32_t tempty_cluster;   // CTA-pair mode: shared::cluster address of the LEADER's tmem-empty barrier (0 = use tempty)
   // this thread's accumulator row
   int n, h, w;
   bool valid;
@@ -213,47 +202,22 @@ struct EpiCtx {
   int bw0, bh0, bn0;
 };
 
-// columns [c0, c0+32) of this thread's row, both accumulator classes summed (fp32, round-to-nearest)
-template <int OFF, int N>
-__device__ __forceinline__ void epi_load32(const EpiCtx& c, int c0, float (&x)[N]) {
-  static_assert(OFF + 32 <= N, "slice out of range");
-  float v[32];
-  ptx::tmem_ld_32x32b_x32_f(c.t_acc + static_cast<uint32_t>(c0), v);
-  if (c.g->n_acc == 2) {
-    float v2[32];
-    ptx::tmem_ld_32x32b_x32_f(c.t_acc + static_cast<uint32_t>(c.g->block_n + c0), v2);
-    ptx::tmem_ld_wait();
+// N columns [c0, c0+N) of this thread's accumulator row into x[OFF..OFF+N)  (c0 a multiple of 4)
+template <int OFF, int N, int M>
+__device__ __forceinline__ void epi_load(const EpiCtx& c, int c0, float (&x)[M]) {
+  static_assert(OFF + N <= M && N % 4 == 0, "slice out of range");
 #pragma unroll
-    for (int j = 0; j < 32; ++j) x[OFF + j] = v[j] + v2[j];
-  } else {
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) x[OFF + j] = v[j];
+  for (int j = 0; j < N / 4; ++j) {
+    const float4 v = *reinterpret_cast<const float4*>(c.acc + ((((c0 >> 2) + j) ^ c.swz) << 2));
+    x[OFF + 4 * j] = v.x; x[OFF + 4 * j + 1] = v.y; x[OFF + 4 * j + 2] = v.z; x[OFF + 4 * j + 3] = v.w;
   }
 }
+// columns [c0, c0+32) of this thread's row
+template <int OFF, int N>
+__device__ __forceinline__ void epi_load32(const EpiCtx& c, int c0, float (&x)[N]) { epi_load<OFF, 32>(c, c0, x); }
 // 16 columns [c0, c0+16) into x[OFF..OFF+15]
 template <int OFF, int N>
-__device__ __forceinline__ void epi_load16(const EpiCtx& c, int c0, float (&x)[N]) {
-  static_assert(OFF + 16 <= N, "slice out of range");
-  float v[16];
-  ptx::tmem_ld_32x32b_x16_f(c.t_acc + static_cast<uint32_t>(c0), v);
-  if (c.g->n_acc == 2) {
-    float v2[16];
-    ptx::tmem_ld_32x32b_x16_f(c.t_acc + static_cast<uint32_t>(c.g->block_n + c0), v2);
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) x[OFF + j] = v[j] + v2[j];
-  } else {
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) x[OFF + j] = v[j];
-  }
-}
-__device__ __forceinline__ void epi_release_tmem(const EpiCtx& c) {
-  ptx::tc_fence_before();
-  if (c.tempty_cluster) ptx::mbar_arrive_cluster(c.tempty_cluster);
-  else ptx::mbar_arrive(c.tempty);
-}
+__device__ __forceinline__ void epi_load16(const EpiCtx& c, int c0, float (&x)[N]) { epi_load<OFF, 16>(c, c0, x); }
 // 32-column chunks [cb, ce) of the tile that column group grp handles
 __device__ __forceinline__ void epi_chunk_range(const GemmGeom& g, int grp, int* cb, int* ce) {
   const int nch = (g.block_n + 31) / 32;          // the last chunk may be 16 columns wide (block_n = 80)
@@ -262,14 +226,167 @@ __device__ __forceinline__ void epi_chunk_range(const GemmGeom& g, int grp, int*
   *ce = min(nch, *cb + per);
 }
 
-// kPair = true is the cta_group::2 build (must be launched as clusters of 2 with g.pair == 1); the default build contains no
-// CTA-pair instruction, so it launches without a cluster attribute.
-template <class Epi, bool kPair = false>
-// 10 warps = up to 3 warps on one SM sub-partition (16 K registers each) -> at most 168 registers per thread
+// k-steps of one (A piece, B piece) product over a 64-wide k-block into accumulator d
+template <int BN>
+__device__ __forceinline__ void gemm_mma_kblock(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t first,
+                                                unsigned fmt16) {
+#pragma unroll
+  for (int k = 0; k < kBlockK / 16; ++k) {
+    // advancing 16 elements (32 B) along K inside the 128 B swizzle row = +2 in the (addr >> 4) field
+    if (fmt16) ptx::wgmma_m64k16<BN, 1>(d, adesc + 2u * k, bdesc + 2u * k, k > 0 ? 1u : first);
+    else ptx::wgmma_m64k16<BN, 0>(d, adesc + 2u * k, bdesc + 2u * k, k > 0 ? 1u : first);
+  }
+}
+
+// One consumer warpgroup (rows 64*wg ..) over all tiles of this CTA: main loop into registers, accumulator tile to shared
+// memory, epilogue.
+template <class Epi, int BN>
+__device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep,
+                                              uint8_t* smem, uint8_t* smem_b, float* acc_smem, uint64_t* full_bar,
+                                              uint64_t* empty_bar, uint64_t* bfull_bar, uint64_t* bempty_bar, EpiCtx& c,
+                                              int wg, int wl, uint16_t mask_peers, uint16_t mask_b, int csize) {
+  const int lane = c.lane;
+  const int stage_bytes = g.halo ? gemm_halo_a_stage_bytes(g) : gemm_stage_bytes(g);
+  const int b_stage_bytes = gemm_b_stage_bytes(g);
+  const int num_kb = g.R * g.S * g.cin_blocks;
+  const int astride = gemm_acc_stride(g);
+  const bool signaller = wl == 0 && lane == 0;     // one arrive per consumer warpgroup on every barrier it releases
+  // slot release: every CTA that writes into the slot (multicast peers) waits for both consumer warpgroups of each reader
+  auto release = [&](uint64_t* bar, uint16_t mask) {
+    if (!signaller) return;
+    if (csize == 1) {
+      ptx::mbar_arrive(bar);
+    } else {
+      for (int r = 0; r < csize; ++r)
+        if (mask & (1u << r)) ptx::mbar_arrive_cluster(ptx::mapa_u32(bar, static_cast<uint32_t>(r)));
+    }
+  };
+  float acc0[BN / 2], acc1[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+  typename Epi::State user_state;                // per-thread state that persists across this CTA's tiles
+  const int row = c.wq * 32 + lane;
+  const int iw = row % g.tw;
+  const int ih = (row / g.tw) % g.th;
+  const int in = row / (g.tw * g.th);
+  const int row0 = c.wq * 32;
+  const int biw = row0 % g.tw, bih = (row0 / g.tw) % g.th, bin = row0 / (g.tw * g.th);
+  int stage = 0, sbi = 0;
+  uint32_t phase = 0, phb = 0;
+  const uint32_t a_rows = static_cast<uint32_t>(wg * 64 * kBlockK * 2);     // this warpgroup's rows of an A tile
+  for (int ti = 0; tile_at(g, ti, &c.tc); ++ti) {
+    uint32_t started = 0;                        // bit a set once accumulator a has received its first MMA
+    if (g.halo) {
+      // ---- halo mode: per channel block one halo patch, nine taps = nine start rows into it (8-row groups = output rows)
+      int pend_b = -1, pend_a = -1;              // slots read by the wgmma group in flight
+      for (int cb = 0; cb < g.cin_blocks; ++cb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes) +
+                            static_cast<uint32_t>(wg * 8 * kHaloPW * kBlockK * 2);
+        for (int tap = 0; tap < 9; ++tap) {
+          ptx::mbar_wait(&bfull_bar[sbi], phb);
+          const uint32_t sb = ptx::smem_u32(smem_b + sbi * b_stage_bytes);
+          const uint32_t a_off = static_cast<uint32_t>(((tap / 3) * kHaloPW + (tap % 3)) * kBlockK * 2);
+          ptx::wgmma_fence();
+          for (int i = 0; i < g.n_mma; ++i) {
+            const uint64_t adesc = ptx::make_kmajor_sw128_desc_sbo(sa + g.mma_a[i] * kHaloPieceBytes + a_off,
+                                                                   kHaloPW * kBlockK * 2);
+            const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb + g.mma_b[i] * g.block_n * kBlockK * 2);
+            const uint32_t a_id = static_cast<uint32_t>(g.mma_acc[i]);
+            const uint32_t first = (started >> a_id) & 1u;
+            started |= 1u << a_id;
+            if (a_id) gemm_mma_kblock<BN>(acc1, adesc, bdesc, first, g.fmt16);
+            else gemm_mma_kblock<BN>(acc0, adesc, bdesc, first, g.fmt16);
+          }
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();                  // the previous group has finished reading its slots
+          if (pend_b >= 0) release(&bempty_bar[pend_b], mask_b);
+          if (pend_a >= 0) release(&empty_bar[pend_a], 1u << (csize > 1 ? ptx::cluster_ctarank() : 0u));
+          pend_b = sbi;
+          pend_a = tap == 8 ? stage : -1;        // the halo patch may be overwritten once the last tap has read it
+          if (++sbi == g.stages_b) { sbi = 0; phb ^= 1u; }
+        }
+        if (++stage == g.stages) { stage = 0; phase ^= 1u; }
+      }
+      ptx::wgmma_wait<0>();
+      release(&bempty_bar[pend_b], mask_b);
+      if (pend_a >= 0) release(&empty_bar[pend_a], 1u << (csize > 1 ? ptx::cluster_ctarank() : 0u));
+    } else {
+      int pend = -1;
+      for (int kb = 0; kb < num_kb + g.res_kb; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
+        const uint32_t sb = sa + g.nA * kTileABytes;
+        const bool res_block = kb >= num_kb && g.res_kind == 0;    // a second conv source uses the normal product list
+        const int n_prod = res_block ? g.n_mma_res : g.n_mma;
+        ptx::wgmma_fence();
+        for (int i = 0; i < n_prod; ++i) {
+          const int pa = res_block ? g.mma_res_a[i] : g.mma_a[i];
+          const int pb = res_block ? 0 : g.mma_b[i];
+          const uint64_t adesc = ptx::make_kmajor_sw128_desc(sa + pa * kTileABytes + a_rows);
+          const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb + pb * g.block_n * kBlockK * 2);
+          const uint32_t a_id = static_cast<uint32_t>(res_block ? g.mma_res_acc[i] : g.mma_acc[i]);
+          const uint32_t first = (started >> a_id) & 1u;     // 0: this accumulator's first MMA of the tile overwrites
+          started |= 1u << a_id;
+          if (a_id) gemm_mma_kblock<BN>(acc1, adesc, bdesc, first, g.fmt16);
+          else gemm_mma_kblock<BN>(acc0, adesc, bdesc, first, g.fmt16);
+        }
+        ptx::wgmma_commit();
+        if (g.stages == 1) {                     // a one-deep ring: the slot is needed back before the next k-block
+          ptx::wgmma_wait<0>();
+          release(&empty_bar[stage], mask_peers);
+        } else {
+          ptx::wgmma_wait<1>();                  // the previous k-block's group is complete: its slot may be refilled
+          if (pend >= 0) release(&empty_bar[pend], mask_peers);
+          pend = stage;
+        }
+        if (++stage == g.stages) { stage = 0; phase ^= 1u; }
+      }
+      ptx::wgmma_wait<0>();
+      if (pend >= 0) release(&empty_bar[pend], mask_peers);
+    }
+    ptx::reg_fence(acc0);
+    ptx::reg_fence(acc1);
+    // ---- accumulator tile (this warpgroup's 64 rows) -> shared memory, then the epilogue reads it row by row
+    ptx::bar_sync(1 + wg, 128);                  // every thread of the warpgroup is done with the previous tile's rows
+    {
+      const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+      const bool two = g.n_acc == 2;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = r0 + 8 * hr;
+          float2 v = make_float2(acc0[4 * j + 2 * hr], acc0[4 * j + 2 * hr + 1]);
+          if (two) { v.x += acc1[4 * j + 2 * hr]; v.y += acc1[4 * j + 2 * hr + 1]; }
+          *reinterpret_cast<float2*>(acc_smem + r * astride + ((((col >> 2) ^ (r & 7))) << 2) + (col & 3)) = v;
+        }
+      }
+    }
+    ptx::bar_sync(1 + wg, 128);
+    c.n = c.tc.n0 + in;
+    c.h = c.tc.h0 + ih;
+    c.w = c.tc.w0 + iw;
+    c.valid = (c.n < g.Nimg) && (c.h < g.Ho) && (c.w < g.Wo);
+    c.pix = (static_cast<long long>(c.n) * g.Ho + c.h) * g.Wo + c.w;
+    c.col0 = c.tc.n_tile * g.block_n;
+    c.bw0 = c.tc.w0 + biw;
+    c.bh0 = c.tc.h0 + bih;
+    c.bn0 = c.tc.n0 + bin;
+    Epi::prefetch(ep, c, user_state);
+    Epi::run(ep, c, user_state);
+    c.prev_m_tile = c.tc.m_tile;
+  }
+  if (lane == 0) ptx::bulk_wait_read0();         // staging tile must outlive the last TMA store's read
+}
+
+template <class Epi>
+// 12 warps = 3 warpgroups -> at most 168 registers per thread
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment is required by the 128B swizzle atoms (TMA writes and UMMA reads must agree on the pattern).
+  // 1024-byte alignment is required by the 128B swizzle atoms (TMA writes and wgmma reads must agree on the pattern).
   // (pointer arithmetic on smem_raw -- not an integer round-trip -- so the compiler keeps the shared address space and
   //  emits LDS/STS instead of generic LD/ST for everything derived from it)
   uint8_t* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -277,19 +394,18 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
   const int b_stage_bytes = gemm_b_stage_bytes(g);                               // halo mode: the weights ring
   uint8_t* smem_b = smem + g.stages * stage_bytes;                              // [stages_b][nB][block_n x 128 B] (halo mode)
   uint8_t* out_stage = smem_b + (g.halo ? g.stages_b * b_stage_bytes : 0);     // [kEpiWarps][4 KiB]
-  uint8_t* extra_smem = out_stage + kEpiWarps * kStageOutBytes;                 // [Epi::kExtraSmemBytes]
+  float* acc_smem = reinterpret_cast<float*>(out_stage + kEpiWarps * kStageOutBytes);   // [128][gemm_acc_stride]
+  uint8_t* extra_smem = out_stage + kEpiWarps * kStageOutBytes + gemm_acc_bytes(g);     // [Epi::kExtraSmemBytes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(extra_smem + Epi::kExtraSmemBytes);
   uint64_t* full_bar = bars;                     // [stages]
   uint64_t* empty_bar = bars + g.stages;         // [stages]
-  uint64_t* tfull_bar = bars + 2 * g.stages;     // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  uint64_t* bfull_bar = tempty_bar + 3;          // [stages_b]   (halo mode)
+  uint64_t* bfull_bar = bars + 2 * g.stages;     // [stages_b]   (halo mode)
   uint64_t* bempty_bar = bfull_bar + 8;          // [stages_b]
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // provably warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
   const int num_kb = g.R * g.S * g.cin_blocks;
+  const int csize = g.cl_m * g.cl_n;
 
   if (warp == 0 && lane == 0) {
     for (int i = 0; i < g.nA; ++i) ptx::prefetch_tmap(&maps.a[i]);
@@ -299,35 +415,18 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
     const int n_peers = g.cl_m + g.cl_n - 1;       // CTAs that read what I multicast == CTAs that multicast to me
     for (int s = 0; s < g.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], (kPair || g.halo) ? 1 : n_peers);   // a slot is free when every consumer of my slices has
-                                                                        // released it (halo patches are never shared)
+      ptx::mbar_init(&empty_bar[s], 2 * (g.halo ? 1 : n_peers));   // both consumer warpgroups of every CTA that reads my
+                                                                    // slices (halo patches are never shared)
     }
     if (g.halo)
       for (int s = 0; s < g.stages_b; ++s) {
         ptx::mbar_init(&bfull_bar[s], 1);
-        ptx::mbar_init(&bempty_bar[s], g.cl_m);     // cluster: every CTA that I multicast weight slices to must release the slot
+        ptx::mbar_init(&bempty_bar[s], 2 * g.cl_m); // cluster: every CTA that I multicast weight slices to must release the slot
       }
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&tfull_bar[b], 1);
-      ptx::mbar_init(&tempty_bar[b], (kPair ? 2 : 1) * kEpiWarps * 32);   // pair: both CTAs' epilogues release the leader's
-    }
     ptx::fence_mbar_init();
   }
-  if (warp == 0) {
-    if constexpr (kPair) {
-      ptx::tmem_alloc_2sm(tmem_slot, kTmemCols);
-      ptx::tmem_relinquish_2sm();
-    } else {
-      ptx::tmem_alloc(tmem_slot, kTmemCols);
-      ptx::tmem_relinquish();
-    }
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // ---- cluster bookkeeping (csize == 1: everything below degenerates to the single-CTA protocol)
-  const int csize = kPair ? 2 : g.cl_m * g.cl_n;
   const int crank = csize > 1 ? static_cast<int>(ptx::cluster_ctarank()) : 0;
   const int ci = crank / g.cl_n, cj = crank % g.cl_n;
   uint16_t mask_a = 0, mask_b = 0;                 // CTAs sharing my row tile (A) / my column tile (B)
@@ -335,8 +434,8 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
   for (int i = 0; i < g.cl_m; ++i) mask_b |= static_cast<uint16_t>(1u << (i * g.cl_n + cj));
   const uint16_t mask_peers = mask_a | mask_b;     // everyone I exchange operand slices with (including myself)
   if (csize > 1) ptx::cluster_sync_all();          // peers' barriers are initialised before anyone signals them
-  // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch) may overlap the previous kernel's tail;
-  // nothing below may touch global memory before the previous grid has fully completed.
+  // PDL: everything above (barrier init, descriptor prefetch) may overlap the previous kernel's tail; nothing below may
+  // touch global memory before the previous grid has fully completed.
   ptx::grid_dep_launch();
   ptx::grid_dep_wait();
 
@@ -404,47 +503,26 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
             uint8_t* st = smem + stage * stage_bytes;
             const int r = kb - num_kb;
             if (ptx::elect_one_sync()) {
-            if constexpr (kPair) {
-              // CTA pair: my A tile and my half of the B rows; every byte of both CTAs is accounted on the leader's barrier
-              const uint32_t lead_full = ptx::mapa_u32(&full_bar[stage], 0);
-              const int b_half = (g.block_n >> 1) * kBlockK * 2;
-              const int b_row = tc.n_tile * g.block_n + crank * (g.block_n >> 1);
-              uint8_t* sb2 = st + g.nA * kTileABytes;
               if (g.res_kind == 0) {
-                if (crank == 0)
-                  ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(2 * (g.nA * kTileABytes + b_half)));
+                // identity residual: A = residual tile (the tile's own channels), B = identity columns (piece 0 only: the
+                // other planes are zero there and are never multiplied)
+                ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(g.nA * kTileABytes + g.block_n * kBlockK * 2));
                 const int rc = tc.n_tile * g.block_n + r * kBlockK;
                 for (int i = 0; i < g.nA; ++i)
-                  ptx::tma_load_4d_2sm(st + i * kTileABytes, &maps.r[i], lead_full, rc, tc.w0, tc.h0, tc.n0);
-                ptx::tma_load_2d_2sm(sb2, &maps.b[0], lead_full, num_kb * kBlockK + rc, b_row);
-              } else {
-                if (crank == 0) ptx::mbar_expect_tx(&full_bar[stage], 2 * tx_bytes);
-                for (int i = 0; i < g.nA; ++i)
-                  ptx::tma_load_4d_2sm(st + i * kTileABytes, &maps.r[i], lead_full, r * kBlockK, tc.w0 * g.res_stride,
-                                       tc.h0 * g.res_stride, tc.n0);
-                for (int i = 0; i < g.nB; ++i)
-                  ptx::tma_load_2d_2sm(sb2 + i * b_half, &maps.b[i], lead_full, (num_kb + r) * kBlockK, b_row);
-              }
-            } else if (g.res_kind == 0) {
-              // identity residual: A = residual tile (the tile's own channels), B = identity columns (piece 0 only: the
-              // other planes are zero there and are never multiplied)
-              ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(g.nA * kTileABytes + g.block_n * kBlockK * 2));
-              const int rc = tc.n_tile * g.block_n + r * kBlockK;
-              for (int i = 0; i < g.nA; ++i)
-                ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], rc, tc.w0, tc.h0, tc.n0);
-              ptx::tma_load_2d(st + g.nA * kTileABytes, &maps.b[0], &full_bar[stage], num_kb * kBlockK + rc,
-                               tc.n_tile * g.block_n);
-            } else {
-              // second 1x1 source: A = 64 channels of the other tensor at (strided) pixel coordinates, B = its weights
-              ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
-              for (int i = 0; i < g.nA; ++i)
-                ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], r * kBlockK, tc.w0 * g.res_stride,
-                                 tc.h0 * g.res_stride, tc.n0);
-              uint8_t* sb2 = st + g.nA * kTileABytes;
-              for (int i = 0; i < g.nB; ++i)
-                ptx::tma_load_2d(sb2 + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], (num_kb + r) * kBlockK,
+                  ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], rc, tc.w0, tc.h0, tc.n0);
+                ptx::tma_load_2d(st + g.nA * kTileABytes, &maps.b[0], &full_bar[stage], num_kb * kBlockK + rc,
                                  tc.n_tile * g.block_n);
-            }
+              } else {
+                // second 1x1 source: A = 64 channels of the other tensor at (strided) pixel coordinates, B = its weights
+                ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
+                for (int i = 0; i < g.nA; ++i)
+                  ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], r * kBlockK, tc.w0 * g.res_stride,
+                                   tc.h0 * g.res_stride, tc.n0);
+                uint8_t* sb2 = st + g.nA * kTileABytes;
+                for (int i = 0; i < g.nB; ++i)
+                  ptx::tma_load_2d(sb2 + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], (num_kb + r) * kBlockK,
+                                   tc.n_tile * g.block_n);
+              }
             }
             __syncwarp();
             if (++stage == g.stages) { stage = 0; phase ^= 1u; }
@@ -461,194 +539,68 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
           uint8_t* sb = st + g.nA * kTileABytes;
           const int kcol = kb * kBlockK;
           if (ptx::elect_one_sync()) {
-          if (!kPair) ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
-          else if (crank == 0) ptx::mbar_expect_tx(&full_bar[stage], 2 * tx_bytes);
-          if constexpr (kPair) {
-            const uint32_t lead_full = ptx::mapa_u32(&full_bar[stage], 0);
-            const int b_half = (g.block_n >> 1) * kBlockK * 2;
-            for (int i = 0; i < g.nA; ++i)
-              ptx::tma_load_4d_2sm(st + i * kTileABytes, &maps.a[i], lead_full, cb * kBlockK, cw, ch, tc.n0);
-            for (int i = 0; i < g.nB; ++i)
-              ptx::tma_load_2d_2sm(sb + i * b_half, &maps.b[i], lead_full, kcol,
-                                   tc.n_tile * g.block_n + crank * (g.block_n >> 1));
-          } else if (csize == 1) {
-            for (int i = 0; i < g.nA; ++i)
-              ptx::tma_load_4d(st + i * kTileABytes, &maps.a[i], &full_bar[stage], cb * kBlockK, cw, ch, tc.n0);
-            for (int i = 0; i < g.nB; ++i)
-              ptx::tma_load_2d(sb + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], kcol,
-                               tc.n_tile * g.block_n);
-          } else {
-            // my 1/cl_n slice of the A rows and 1/cl_m slice of the B rows, multicast to the CTAs that share them
-            const int a_rows = kBlockM / g.cl_n, b_rows = g.block_n / g.cl_m;
-            for (int i = 0; i < g.nA; ++i)
-              ptx::tma_load_4d_mc(st + i * kTileABytes + cj * a_rows * kBlockK * 2, &maps.a[i], &full_bar[stage],
-                                  cb * kBlockK, cw + cj * a_rows, ch, tc.n0, mask_a);
-            for (int i = 0; i < g.nB; ++i)
-              ptx::tma_load_2d_mc(sb + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2, &maps.b[i],
-                                  &full_bar[stage], kcol, tc.n_tile * g.block_n + ci * b_rows, mask_b);
-          }
-          }
-          __syncwarp();
-          if (++stage == g.stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (whole warp walks the schedule, one elected lane issues)
-    if (!kPair || crank == 0) {
-      const uint32_t idesc = ptx::make_idesc_f16(g.fmt16, kPair ? 2 * kBlockM : kBlockM, static_cast<uint32_t>(g.block_n));
-      const int b_piece_bytes = (g.block_n >> (kPair ? 1 : 0)) * kBlockK * 2;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      TileCoord tc_unused;
-      int sbi = 0;
-      uint32_t phb = 0;
-      for (int ti = 0; g.halo && tile_at(g, ti, &tc_unused); ++ti) {
-        // ---- halo mode: per channel block one halo patch, nine taps = nine start rows into it
-        ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * g.n_acc * g.block_n);
-        uint32_t started = 0;
-        for (int cb = 0; cb < g.cin_blocks; ++cb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
-          for (int tap = 0; tap < 9; ++tap) {
-            ptx::mbar_wait(&bfull_bar[sbi], phb);
-            ptx::tc_fence_after();
-            const uint32_t sb = ptx::smem_u32(smem_b + sbi * b_stage_bytes);
-            const uint32_t a_off = static_cast<uint32_t>(((tap / 3) * kHaloPW + (tap % 3)) * kBlockK * 2);
-            for (int i = 0; i < g.n_mma; ++i) {
-              const uint64_t adesc = ptx::make_kmajor_sw128_desc_sbo(sa + g.mma_a[i] * kHaloPieceBytes + a_off,
-                                                                     kHaloPW * kBlockK * 2);
-              const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb + g.mma_b[i] * g.block_n * kBlockK * 2);
-              const uint32_t a_id = static_cast<uint32_t>(g.mma_acc[i]);
-              const uint32_t d_acc = d_tmem + a_id * static_cast<uint32_t>(g.block_n);
-              const uint32_t first = (started >> a_id) & 1u;
-              started |= 1u << a_id;
-              if (ptx::elect_one_sync()) {
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k)
-                  ptx::umma_f16(d_acc, adesc + 2u * k, bdesc + 2u * k, idesc, k > 0 ? 1u : first);
-              }
-              __syncwarp();
-            }
-            if (ptx::elect_one_sync()) {
-              if (csize == 1) ptx::umma_commit(&bempty_bar[sbi]);
-              else ptx::umma_commit_mc(&bempty_bar[sbi], mask_b);     // every CTA that writes into my slot
-              if (tap == 8) ptx::umma_commit(&empty_bar[stage]);   // the halo patch may be overwritten once these MMAs have read it
-              if (tap == 8 && cb == g.cin_blocks - 1) ptx::umma_commit(&tfull_bar[acc]);
-            }
-            __syncwarp();
-            if (++sbi == g.stages_b) { sbi = 0; phb ^= 1u; }
-          }
-          if (++stage == g.stages) { stage = 0; phase ^= 1u; }
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
-      }
-      for (int ti = 0; !g.halo && tile_at(g, ti, &tc_unused); ++ti) {
-        ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * g.n_acc * g.block_n);
-        uint32_t started = 0;                        // bit a set once accumulator a has received its first MMA
-        for (int kb = 0; kb < num_kb + g.res_kb; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tc_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
-          const uint32_t sb = sa + g.nA * kTileABytes;
-          const bool res_block = kb >= num_kb && g.res_kind == 0;    // a second conv source uses the normal product list
-          const int n_prod = res_block ? g.n_mma_res : g.n_mma;
-          for (int i = 0; i < n_prod; ++i) {
-            const int pa = res_block ? g.mma_res_a[i] : g.mma_a[i];
-            const int pb = res_block ? 0 : g.mma_b[i];
-            const uint64_t adesc = ptx::make_kmajor_sw128_desc(sa + pa * kTileABytes);
-            const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb + pb * b_piece_bytes);
-            const uint32_t a_id = static_cast<uint32_t>(res_block ? g.mma_res_acc[i] : g.mma_acc[i]);
-            const uint32_t d_acc = d_tmem + a_id * static_cast<uint32_t>(g.block_n);
-            const uint32_t first = (started >> a_id) & 1u;     // 0: this accumulator's first MMA of the tile overwrites
-            started |= 1u << a_id;
-            if (ptx::elect_one_sync()) {
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k) {
-                // advancing 16 elements (32 B) along K inside the 128 B swizzle row = +2 in the (addr >> 4) field
-                if constexpr (kPair) ptx::umma_f16_2sm(d_acc, adesc + 2u * k, bdesc + 2u * k, idesc, k > 0 ? 1u : first);
-                else ptx::umma_f16(d_acc, adesc + 2u * k, bdesc + 2u * k, idesc, k > 0 ? 1u : first);
-              }
-            }
-            __syncwarp();
-          }
-          const bool last_kb = kb == num_kb + g.res_kb - 1;
-          if (ptx::elect_one_sync()) {
-            if constexpr (kPair) ptx::umma_commit_2sm_mc(&empty_bar[stage], 3);   // both CTAs' slots were read by these MMAs
-            else if (csize == 1) ptx::umma_commit(&empty_bar[stage]);   // smem slot reusable once these MMAs have read it
-            else ptx::umma_commit_mc(&empty_bar[stage], mask_peers);   // ... tell every CTA that fills this slot
-            if (last_kb) {
-              if constexpr (kPair) ptx::umma_commit_2sm_mc(&tfull_bar[acc], 3);   // both halves of the accumulator are complete
-              else ptx::umma_commit(&tfull_bar[acc]);   // accumulator complete
+            ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
+            if (csize == 1) {
+              for (int i = 0; i < g.nA; ++i)
+                ptx::tma_load_4d(st + i * kTileABytes, &maps.a[i], &full_bar[stage], cb * kBlockK, cw, ch, tc.n0);
+              for (int i = 0; i < g.nB; ++i)
+                ptx::tma_load_2d(sb + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], kcol,
+                                 tc.n_tile * g.block_n);
+            } else {
+              // my 1/cl_n slice of the A rows and 1/cl_m slice of the B rows, multicast to the CTAs that share them
+              const int a_rows = kBlockM / g.cl_n, b_rows = g.block_n / g.cl_m;
+              for (int i = 0; i < g.nA; ++i)
+                ptx::tma_load_4d_mc(st + i * kTileABytes + cj * a_rows * kBlockK * 2, &maps.a[i], &full_bar[stage],
+                                    cb * kBlockK, cw + cj * a_rows, ch, tc.n0, mask_a);
+              for (int i = 0; i < g.nB; ++i)
+                ptx::tma_load_2d_mc(sb + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2, &maps.b[i],
+                                    &full_bar[stage], kcol, tc.n_tile * g.block_n + ci * b_rows, mask_b);
             }
           }
           __syncwarp();
           if (++stage == g.stages) { stage = 0; phase ^= 1u; }
         }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
       }
     }
   } else if (warp >= kFirstEpiWarp) {
-    // ===================================================== epilogue warps
-    typename Epi::State user_state;                // per-thread state that persists across this CTA's tiles
+    // ===================================================== consumer warpgroups: wgmma main loop + epilogue
+    const int wg = (warp - kFirstEpiWarp) >> 2;
+    const int wl = warp & 3;
     EpiCtx c;
     c.g = &g;
     c.maps = &maps;
-    c.wq = warp & 3;
-    c.grp = (warp - kFirstEpiWarp) >> 2;
+    c.wq = 2 * wg + (wl & 1);
+    c.grp = wl >> 1;
     c.lane = lane;
+    const int row = c.wq * 32 + lane;
+    c.acc = acc_smem + row * gemm_acc_stride(g);
+    c.swz = row & 7;
     c.stage = out_stage + (warp - kFirstEpiWarp) * kStageOutBytes;
     c.extra = extra_smem;
     c.prev_m_tile = -1;
     c.store_seq = 0;
-    const int row = c.wq * 32 + lane;
-    const int iw = row % g.tw;
-    const int ih = (row / g.tw) % g.th;
-    const int in = row / (g.tw * g.th);
-    const int row0 = c.wq * 32;
-    const int biw = row0 % g.tw, bih = (row0 / g.tw) % g.th, bin = row0 / (g.tw * g.th);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int ti = 0; tile_at(g, ti, &c.tc); ++ti) {
-      c.n = c.tc.n0 + in;
-      c.h = c.tc.h0 + ih;
-      c.w = c.tc.w0 + iw;
-      c.valid = (c.n < g.Nimg) && (c.h < g.Ho) && (c.w < g.Wo);
-      c.pix = (static_cast<long long>(c.n) * g.Ho + c.h) * g.Wo + c.w;
-      c.col0 = c.tc.n_tile * g.block_n;
-      c.bw0 = c.tc.w0 + biw;
-      c.bh0 = c.tc.h0 + bih;
-      c.bn0 = c.tc.n0 + bin;
-      c.tempty = &tempty_bar[acc];
-      c.tempty_cluster = kPair ? ptx::mapa_u32(&tempty_bar[acc], 0) : 0u;
-      c.t_acc = tmem_base + (static_cast<uint32_t>(c.wq * 32) << 16) + static_cast<uint32_t>(acc * g.n_acc * g.block_n);
-      Epi::prefetch(ep, c, user_state);            // global reads that do not depend on the accumulator overlap the main loop
-      ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-      ptx::tc_fence_after();
-      Epi::run(ep, c, user_state);                 // must call epi_release_tmem(c) exactly once per thread
-      c.prev_m_tile = c.tc.m_tile;
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1u;
+    switch (g.block_n) {
+      case 64:
+        gemm_consumer<Epi, 64>(maps, g, ep, smem, smem_b, acc_smem, full_bar, empty_bar, bfull_bar, bempty_bar, c, wg, wl,
+                               mask_peers, mask_b, csize);
+        break;
+      case 80:
+        gemm_consumer<Epi, 80>(maps, g, ep, smem, smem_b, acc_smem, full_bar, empty_bar, bfull_bar, bempty_bar, c, wg, wl,
+                               mask_peers, mask_b, csize);
+        break;
+      case 96:
+        gemm_consumer<Epi, 96>(maps, g, ep, smem, smem_b, acc_smem, full_bar, empty_bar, bfull_bar, bempty_bar, c, wg, wl,
+                               mask_peers, mask_b, csize);
+        break;
+      default:
+        gemm_consumer<Epi, 128>(maps, g, ep, smem, smem_b, acc_smem, full_bar, empty_bar, bfull_bar, bempty_bar, c, wg, wl,
+                                mask_peers, mask_b, csize);
+        break;
     }
-    if (lane == 0) ptx::bulk_wait_read0();         // staging tile must outlive the last TMA store's read
   }
 
-  ptx::tc_fence_before();
   __syncthreads();
   if (csize > 1) ptx::cluster_sync_all();          // nobody leaves while a peer may still write my smem / barriers
-  if (warp == 0) {
-    ptx::tc_fence_after();
-    if constexpr (kPair) ptx::tmem_dealloc_2sm(tmem_base, kTmemCols);
-    else ptx::tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 }  // namespace dad3d

@@ -148,7 +148,7 @@ class Dad3dEncoder:
     def __init__(self, state_dict: Dict[str, Tensor], device: Optional[torch.device] = None, precision: str = "fp32",
                  want_heatmap: bool = True):
         if not torch.cuda.is_available():
-            raise _lib.Dad3dError("dad_3dheads_b200 needs a CUDA (sm_100a) device: there is no CPU path")
+            raise _lib.Dad3dError("dad_3dheads_b200 needs a CUDA (sm_90a) device: there is no CPU path")
         self.lib = _lib.load()
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         if self.device.type != "cuda":

@@ -32,7 +32,7 @@ class DADEvaluatorGPU:
     def __init__(self, ground_truth_path: Optional[str] = None, submission_path: Optional[str] = None, cuda_id: int = 0,
                  static: Optional[Dict[str, np.ndarray]] = None):
         if not torch.cuda.is_available():
-            raise _lib.Dad3dError("DADEvaluatorGPU needs a CUDA (sm_100a) device: there is no CPU path")
+            raise _lib.Dad3dError("DADEvaluatorGPU needs a CUDA (sm_90a) device: there is no CPU path")
         self.lib = _lib.load()
         self.device = torch.device("cuda", cuda_id)
         self.target_file_path = ground_truth_path

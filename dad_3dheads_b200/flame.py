@@ -107,7 +107,7 @@ class FlameDecoder:
 
     def __init__(self, static: Dict[str, np.ndarray], consts: Dict[str, int], device: torch.device):
         if not torch.cuda.is_available():
-            raise _lib.Dad3dError("dad_3dheads_b200 needs a CUDA (sm_100a) device: there is no CPU path")
+            raise _lib.Dad3dError("dad_3dheads_b200 needs a CUDA (sm_90a) device: there is no CPU path")
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -182,7 +182,7 @@ class FlameDecoder:
     def backward(self, params: Tensor, grad_vertices: Optional[Tensor], grad_projected: Optional[Tensor], *, to_2d: bool = True,
                  zero_rot: bool = False, zero_jaw: bool = False, image_size: float = 256.0) -> Tensor:
         """d L / d params [B, num_params] from d L / d vertices3d [B,V,3] and / or d L / d projected [B,V,2|3] (either may be
-        None): the backward of :meth:`decode` (csrc/flame.cu ``dad3d_flame_backward``; dense part on tcgen05)."""
+        None): the backward of :meth:`decode` (csrc/flame.cu ``dad3d_flame_backward``; dense part on wgmma)."""
         assert params.is_cuda and params.dtype == torch.float32 and params.ndim == 2 and params.shape[1] == self.num_params
         assert grad_vertices is not None or grad_projected is not None
         params = params.contiguous()
@@ -295,7 +295,7 @@ class FLAMELayer(nn.Module):
     def decoder(self, device: Optional[torch.device] = None) -> FlameDecoder:
         if device is None or torch.device(device).type != "cuda":
             if not torch.cuda.is_available():
-                raise _lib.Dad3dError("FLAMELayer needs a CUDA (sm_100a) device: there is no CPU path")
+                raise _lib.Dad3dError("FLAMELayer needs a CUDA (sm_90a) device: there is no CPU path")
             idx = self._cuda_id if self._cuda_id is not None else torch.cuda.current_device()
         else:
             device = torch.device(device)

@@ -87,7 +87,7 @@ class FaceMeshPredictor:
     def __init__(self, config: Dict[str, Any], cuda_id: int = 0, state_dict: Optional[Dict[str, Tensor]] = None,
                  precision: str = "fp32"):
         if not torch.cuda.is_available():
-            raise _lib.Dad3dError("FaceMeshPredictor needs a CUDA (sm_100a) device: there is no CPU path")
+            raise _lib.Dad3dError("FaceMeshPredictor needs a CUDA (sm_90a) device: there is no CPU path")
         self.cuda_id = cuda_id
         self.device = torch.device("cuda", cuda_id)
         self.flame_constants = config["constants"]

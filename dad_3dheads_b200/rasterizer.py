@@ -13,7 +13,7 @@ from . import _lib
 
 def _device(cuda_id: Optional[int]) -> torch.device:
     if not torch.cuda.is_available():
-        raise _lib.Dad3dError("dad_3dheads_b200.rasterizer needs a CUDA (sm_100a) device: there is no CPU path")
+        raise _lib.Dad3dError("dad_3dheads_b200.rasterizer needs a CUDA (sm_90a) device: there is no CPU path")
     return torch.device("cuda", torch.cuda.current_device() if cuda_id is None else cuda_id)
 
 

@@ -1,4 +1,4 @@
-/* libdad3d.so -- C ABI of the B200-native DAD-3DNet image->3D-head hot path.
+/* libdad3d.so -- C ABI of the H100-native DAD-3DNet image->3D-head hot path.
  *
  * The reference (PinataFarms/DAD-3DHeads) has no FFI seam: its "operator interface" for this path is three Python
  * objects (SURVEY.md §8b).  Each entry point below names the reference call it replaces (file:line under
@@ -35,7 +35,7 @@ typedef struct dad3d_encoder dad3d_encoder;
 #define DAD3D_ERR_UNSUPPORTED (-3)
 
 #define DAD3D_DECODE_CLUSTER 32 /* A/B aid: fused decode as 2x2 thread-block clusters with TMA multicast of both operands
-                                  (measured slower on B200, so off by default) */
+                                  (off by default) */
 
 /* Widths of the fields of the 3DMM parameter vector, sliced in the reference's hard-coded order
  * shape, expression, jaw, rotation, eyeballs, neck, translation, scale
@@ -51,10 +51,8 @@ typedef struct dad3d_flame_layout {
 #define DAD3D_BLEND_HILO 64     /* blend-shape product with fp16 hi/lo split operands (3 tensor-core products, 22-bit, vertices
                                    relL2 2e-7 vs fp64) through the generic tile engine.  DEFAULT (flag absent): ONE fp16 product
                                    (11-bit operand mantissa like TF32, template exact to 22 bits; vertices relL2 1.5e-5, inside
-                                   the 1e-4 contract) in the dedicated A-stationary decode kernel (csrc/flame_decode.cuh) */
-#define DAD3D_DECODE_PAIR 128   /* run the dedicated decode kernel as CTA pairs (cta_group::2) when the batch has at least two row
-                                   tiles per SM.  Pairs are the default there since round 2 (environment DAD3D_DECODE_PAIR=0
-                                   switches them off for A/B runs); the flag forces them regardless of the environment */
+                                   the 1e-4 contract) in the dedicated decode kernel (csrc/flame_decode.cuh) */
+#define DAD3D_DECODE_PAIR 128   /* accepted, no effect: CTA pairs need a two-CTA MMA, which sm_90 lacks */
 #define DAD3D_BLEND_SIMT 8      /* verification aid: blend-shape product on CUDA cores in fp32 (slow) */
 #define DAD3D_DECODE_UNFUSED 16 /* A/B aid: tensor-core blend product to a v_posed scratch + separate skinning kernel
                                    (default: skinning / rotation / projection fused into the GEMM epilogue) */
@@ -95,7 +93,7 @@ DAD3D_API int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t 
  * grad_vertices_d [B,V,3] = dL/d(vertices3d) and / or grad_projected_d [B,V,2|3] = dL/d(projected) (either may be NULL).
  * What autograd gives the reference when its losses call HeadMesh.vertices_3d / reprojected_vertices
  * (losses/vertices_3d_loss.py:30-47, losses/reprojection_loss.py:22-46, train/flame_lightning_model.py:329-351).  The dense
- * part (d beta, d pose features) is a tcgen05 GEMM over the transposed basis; layouts without neck / eyeball pose only. */
+ * part (d beta, d pose features) is a wgmma GEMM over the transposed basis; layouts without neck / eyeball pose only. */
 DAD3D_API size_t dad3d_flame_backward_workspace_bytes(const dad3d_flame* h, int32_t B);
 DAD3D_API int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, const float* grad_vertices_d,
                                    const float* grad_projected_d, float image_size, int32_t to_2d, float* grad_params_d,
@@ -169,7 +167,7 @@ DAD3D_API int dad3d_preprocess_batch(const uint8_t* images_d, int32_t B, int32_t
                                      int32_t img_size, const float* mean255_h, const float* inv_std255_h, float* out_d,
                                      dad3d_stream stream);
 
-/* Live timing of the dominant kernel (the tcgen05 tile engine) for bench.py's roofline: while on, every conv / linear
+/* Live timing of the dominant kernel (the wgmma tile engine) for bench.py's roofline: while on, every conv / linear
  * launch is bracketed by CUDA events on the launching stream.  profile_read synchronises those events and returns their
  * summed duration, the launch count and the ALGORITHMIC FLOPs (2 * true MACs, one product per MAC, no padding) of the
  * recorded launches, then resets the counters. */

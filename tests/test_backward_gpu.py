@@ -1,7 +1,7 @@
 """-m gpu: the decoder backward (dad3d_flame_backward through the C ABI) against torch.autograd through the fp64 oracle
 (oracle/flame_oracle.py, itself pinned to the reference's FLAMELayer / HeadMesh): gradients of a random linear functional of
 (vertices_3d, reprojected_vertices) w.r.t. all 413 parameters.  Tolerance: relL2 < 1e-4 per parameter group (measured ~1e-6;
-the forward blend inside is the 3-product hi/lo GEMM, the dense backward part a 3-product tcgen05 GEMM)."""
+the forward blend inside is the 3-product hi/lo GEMM, the dense backward part a 3-product wgmma GEMM)."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""-m gpu: the reference's OWN demo.py / demo_utils.py, unmodified, over the B200 path (north_star: "keeping
+"""-m gpu: the reference's OWN demo.py / demo_utils.py, unmodified, over the H100 path (north_star: "keeping
 predictor.FaceMeshPredictor's API so demo.py ... run unchanged").
 
 ``sys.path`` = [compat/ (predictor, model_training, utils, Sim3DR -> libdad3d.so), oracle/ref_shims (stand-ins for the

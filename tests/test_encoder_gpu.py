@@ -113,24 +113,11 @@ def test_batch_64_matches_oracle_subset(sd, cuda_device):
     assert torch.isfinite(p).all()
 
 
-def test_cta_pair_mode_is_bit_identical(sd, cuda_device, monkeypatch):
-    """DAD3D_PAIR=1 runs the large layers on cta_group::2 CTA pairs (256-row tiles, B split across the pair): the same
-    products in the same order, so the outputs must equal the single-CTA path bit for bit (batch 64: pairs only engage
-    when every SM pair has work)."""
-    from dad_3dheads_b200.encoder import Dad3dEncoder
-    x = torch.randn(64, 3, 256, 256, generator=torch.Generator().manual_seed(65)).to(cuda_device)
-    base = Dad3dEncoder(sd, cuda_device, precision="fp16x2", want_heatmap=False).forward_raw(x)
-    monkeypatch.setenv("DAD3D_PAIR", "1")
-    pair = Dad3dEncoder(sd, cuda_device, precision="fp16x2", want_heatmap=False).forward_raw(x)
-    monkeypatch.delenv("DAD3D_PAIR")
-    assert torch.equal(base[0], pair[0]) and torch.equal(base[1], pair[1])
-
-
 @pytest.mark.parametrize("precision,tol", [("fp16x2", 5e-5), ("bf16", 2e-2)])
 @pytest.mark.parametrize("halo", ["1", "0"])
 def test_halo_and_per_tap_paths_match_oracle(sd, ref5, cuda_device, monkeypatch, precision, tol, halo):
     """Default (DAD3D_HALO unset / 1): the 3x3 stride-1 layers run on 8x16-pixel tiles whose nine taps read one shared halo
-    patch through shifted UMMA descriptors (k order: channel block outer, tap inner); DAD3D_HALO=0: one TMA box per tap
+    patch through shifted wgmma descriptors (k order: channel block outer, tap inner); DAD3D_HALO=0: one TMA box per tap
     (tap outer).  Both against the oracle, with the 3x3 layers checked one by one."""
     from dad_3dheads_b200.encoder import Dad3dEncoder, fold_state_dict
     from tests.folded_ref import run_folded

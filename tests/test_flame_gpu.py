@@ -178,8 +178,7 @@ def test_chunk_boundary_and_batch_independence(head_mesh, cuda_device):
     vb, pb = dec.decode(p[:n], want_vertices=True, want_projected=True, cluster=True)
     assert torch.equal(va, vb) and torch.equal(pa, pb)
     del va, pa, vb, pb
-    # CTA pairs (cta_group::2; the default for batches with >= 2 row tiles per SM) against single CTAs (DAD3D_DECODE_PAIR=0,
-    # read at every call) -- same arithmetic
+    # DAD3D_DECODE_PAIR (CTA pairs; no effect on sm_90) and the DAD3D_DECODE_PAIR=0 environment leave the results unchanged
     import os
     n = props.multi_processor_count * 128 * 2 + 77
     old_env = os.environ.get("DAD3D_DECODE_PAIR")

@@ -62,7 +62,7 @@ def test_index_file_readers(tmp_path):
 
 def test_decode_row_permutation_is_a_bijection_with_equal_residues_per_warp():
     """flame_decode.cuh ``dec_phys_row`` / ``dec_head_of`` (restated): physical coefficient row of head h inside its 256-head
-    block = 128 t + 32 wq + l with residue h mod 8 = 4 t + wq, l = (h mod 256) / 8 -- every TMEM lane quarter of a row tile holds
+    block = 128 t + 32 wq + l with residue h mod 8 = 4 t + wq, l = (h mod 256) / 8 -- every accumulator row quarter of a row tile holds
     32 heads that are equal mod 8 (the premise of the per-lane sector-aligned stores)."""
     def phys(h):
         return (h & ~255) + ((h & 7) >> 2) * 128 + (h & 3) * 32 + ((h & 255) >> 3)
