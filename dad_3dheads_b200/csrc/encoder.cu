@@ -469,6 +469,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     const int Wo = s.stem ? ti.W - kS2dPadW : s.parity ? ti.W / 2 : (ti.W + 2 * s.pad - w->S) / s.stride + 1;
     GemmGeom& g = s.geom;
     std::memset(&g, 0, sizeof(g));
+    g.frag_epi = s.out >= 0 ? 1 : 0;                  // piece outputs: fragment epilogue, no shared-memory accumulator tile
     pick_tile(Wo, Ho, &g.tw, &g.th, &g.tn);
     // 3x3 / stride 1 / pad 1 layers: 8 x 16-pixel tiles whose nine taps share one halo patch in shared memory (tile_gemm.cuh
     // "halo mode"); needs a map of at least 8 x 16 pixels and room for a two-deep weights ring (checked below)
@@ -477,7 +478,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     if (halo) {                                       // two halo patches + at least two weight tiles must fit (bf16x3 at N = 128 does not)
       GemmGeom probe;
       std::memset(&probe, 0, sizeof(probe));
-      probe.nA = enc->P; probe.nB = enc->P; probe.block_n = w->block_n;
+      probe.nA = enc->P; probe.nB = enc->P; probe.block_n = w->block_n; probe.frag_epi = g.frag_epi;
       halo = gemm_halo_b_stages(probe) >= 2;
     }
     if (s.sparse_rows) halo = false;                  // row-pair tiles (2 rows x 64 columns) through the per-tap path
@@ -512,7 +513,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
     GemmGeom fit;                                     // the full-width tile needs a two-deep operand ring in shared memory
     std::memset(&fit, 0, sizeof(fit));
-    fit.nA = enc->P; fit.nB = enc->P; fit.block_n = w->block_n;
+    fit.nA = enc->P; fit.nB = enc->P; fit.block_n = w->block_n; fit.frag_epi = g.frag_epi;
     const bool narrow = w->has_b64 && (m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms || gemm_max_stages(fit) < 2);
     const int block_n = narrow ? 64 : w->block_n;
     g.block_n = block_n;
@@ -521,7 +522,6 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     g.n_mma = enc->n_mma;
     g.n_acc = enc->n_acc;
     for (int i = 0; i < enc->n_mma; ++i) { g.mma_a[i] = enc->mma_a[i]; g.mma_b[i] = enc->mma_b[i]; g.mma_acc[i] = enc->mma_acc[i]; }
-    g.fmt16 = enc->fp16 ? 0u : 1u;
     if (res_in_k) {                                   // "+ identity(x)" performed by the tensor core
       g.res_kb = block_n / kBlockK;
       g.n_mma_res = enc->P;
@@ -600,11 +600,11 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
         set_error("layer " + w->name + ": piece outputs need block_n 64 or 128");
         return DAD3D_ERR_INVALID;
       }
-      // per-warp store box: 32 consecutive tile rows = (bw x bh x bn) output pixels x 32 channels (SWIZZLE_64B rows)
+      // per-warp store box: 16 consecutive tile rows = (bw x bh x bn) output pixels x 32 channels (SWIZZLE_64B rows)
       const int nc = 32;
-      const int bw = std::min(g.tw, 32);
-      const int bh = std::min(g.th, 32 / bw);
-      const int bn = 32 / (bw * bh);
+      const int bw = std::min(g.tw, 16);
+      const int bh = std::min(g.th, 16 / bw);
+      const int bn = 16 / (bw * bh);
       for (int p = 0; p < to.planes; ++p) {
         uint16_t* basep = reinterpret_cast<uint16_t*>(to.ptr) + static_cast<size_t>(p) * to.plane_elems();
         if (s.up2 || s.parity) {

@@ -1,5 +1,5 @@
 // Device code of the DAD-3DNet encoder (everything that is not the wgmma tile engine itself):
-//   EpiConv            fused conv epilogue: folded-BN bias, residual add / gate multiply, ReLU, split into bf16 pieces
+//   EpiConvT           fused conv epilogue: folded-BN bias, residual add / gate multiply, ReLU, split into pieces
 //   stem_conv_kernel   7x7/2 conv (Cin = 3) + folded BN + ReLU, fp32 CUDA cores, NCHW fp32 image -> NHWC fp32 (DAD3D_STEM_SIMT=1)
 //   stem_s2d_kernel    2x2 space-to-depth + piece split of the image: the stem runs on the tile engine as a 4x4 conv
 //   stem_pool_kernel   3x3/2 max-pool + split into pieces
@@ -18,7 +18,7 @@
 namespace dad3d {
 
 // ------------------------------------------------------------------------------------------------ piece helpers
-// Two 16-bit piece formats (GemmGeom::fmt16): bf16 (x = p0 + p1 + p2, 8 + 8 + 8 mantissa bits, fp32 exponent range) and
+// Two 16-bit piece formats (EpiConvT<F16>::kBf16): bf16 (x = p0 + p1 + p2, 8 + 8 + 8 mantissa bits, fp32 exponent range) and
 // fp16 (x = hi + lo, 11 + 11 bits; |x| saturates at 65504 and the lo piece goes subnormal below |x| = 2^-3, leaving an
 // absolute representation error <= 2^-25).
 __device__ __forceinline__ uint16_t bf16_bits(float x) { return __bfloat16_as_ushort(__float2bfloat16_rn(x)); }
@@ -131,10 +131,9 @@ struct EpiConvParams {
 template <bool F16>
 struct EpiConvT {
   static constexpr int kExtraSmemBytes = 0;
+  static constexpr int kBf16 = F16 ? 0 : 1;       // operand format of the tile engine
+  static constexpr bool kFragment = true;         // piece outputs (ep.out != nullptr) run on the register fragments
   struct State {};
-  struct Res {
-    float r[64];              // residual / gate operand of the current tile (this thread's row, this warp's columns)
-  };
   using Params = EpiConvParams;
   // fp32-only outputs (heat-map, MLP logits): direct vector stores of this thread's row
   static __device__ __forceinline__ void run_f32(const Params& ep, const EpiCtx& c) {
@@ -168,147 +167,91 @@ struct EpiConvT {
     }
   }
 
-  // The warp's columns are handled in halves of 32 channels (block_n 128 -> two halves per warp, block_n 64 -> one), which
-  // keeps the per-thread working set at 32 accumulator values (+ the prefetched residual).  Staging rows are 64 bytes
-  // (TMA SWIZZLE_64B pattern: 16-byte chunk index XOR ((row >> 1) & 3)).
-  static __device__ __forceinline__ int halves(const EpiCtx& c) { return c.g->block_n / 64; }
-  static __device__ __forceinline__ int first_col(const EpiCtx& c, int half) {
-    return c.grp * (c.g->block_n / 2) + half * 32;            // column inside the tile
-  }
-
-  // Residual / gate operand: the warp's 32 rows x 32 channels per piece plane.  Loads are cooperative (a warp instruction covers whole 64-byte
-  // row segments -> 8 memory wavefronts instead of 32 for per-thread rows), transposed through the staging tile; every
-  // lane then reads back its own row and sums the pieces (smallest first).
-  template <int H>
-  static __device__ __forceinline__ void prefetch_half(const Params& ep, const EpiCtx& c, Res& st) {
-    const int swz = (c.lane >> 1) & 3;
-    const uint8_t* rowp = c.stage + c.lane * 64;
-    const int col = c.col0 + first_col(c, H);
-    // 1) every global load of this half (up to 3 planes x 4 row-segment sweeps) is issued before anything waits on one:
-    //    a single memory round trip instead of one per plane
-    uint4 q[3][4];
-    const int planes = ep.res.planes;
-    const long long rpix = c.pix;                      // this lane's row in the residual tensor
+  // Piece outputs: the fragment epilogue.  Each thread holds rows r0, r0 + 8 of its warp's 16 tile rows and the column
+  // pairs 8j + 2(lane & 3) of the wgmma accumulators; per element, in this order: acc0 + acc1, folded-BN scale and bias,
+  // residual add or gate multiply, ReLU, split into 16-bit pieces.  Columns go in chunks of 32: per piece plane a chunk is
+  // one 1 KiB staging tile (16 rows x 64 B, TMA SWIZZLE_64B pattern: 16-byte chunk index XOR ((row >> 1) & 3), written
+  // bank-conflict free with 32-bit stores) and one TMA store of the warp's 16-row box.
+  template <int BN>
+  static __device__ __forceinline__ void run_frag(const Params& ep, FragCtx& f, const float (&a0)[BN / 2],
+                                                  const float (&a1)[BN / 2], bool two) {
+    const int q = f.lane & 3;
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      const int idx = it * 32 + c.lane;
-      const int row = idx >> 2, seg = idx & 3;
-      const long long spix = __shfl_sync(0xffffffffu, rpix, row);
-      const int svalid = __shfl_sync(0xffffffffu, c.valid ? 1 : 0, row);
-      const uint16_t* src = ep.res.base + spix * ep.res.C + col + seg * 8;
+    for (int ch = 0; ch < BN / 32; ++ch) {
+      float x[16];                                     // the chunk's values: x[4 jj + 2 hr + e] = a0[4 (4 ch + jj) + 2 hr + e]
 #pragma unroll
-      for (int p = 0; p < 3; ++p) {
-        q[p][it] = make_uint4(0, 0, 0, 0);
-        if (p < planes && svalid) q[p][it] = __ldg(reinterpret_cast<const uint4*>(src + p * ep.res.plane));
-      }
-    }
-    if (c.lane == 0) ptx::bulk_wait_read0();          // an earlier TMA store may still be reading the staging tile
-    __syncwarp();
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * ch + jj;
+        const int col = f.col0 + 8 * j + 2 * q;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
+        float2 sc = make_float2(1.f, 1.f);
+        if constexpr (F16) sc = __ldg(reinterpret_cast<const float2*>(ep.scale + col));
 #pragma unroll
-    for (int j = 0; j < 32; ++j) st.r[H * 32 + j] = 0.f;
-    // 2) transpose plane by plane through the staging tile (smallest piece first) and sum this lane's row
+        for (int hr = 0; hr < 2; ++hr) {
+          float& x0 = x[4 * jj + 2 * hr];
+          float& x1 = x[4 * jj + 2 * hr + 1];
+          x0 = a0[4 * j + 2 * hr];
+          x1 = a0[4 * j + 2 * hr + 1];
+          if (two) { x0 += a1[4 * j + 2 * hr]; x1 += a1[4 * j + 2 * hr + 1]; }
+          if constexpr (F16) {
+            x0 = fmaf(x0, sc.x, b.x); x1 = fmaf(x1, sc.y, b.y);
+          } else {
+            x0 += b.x; x1 += b.y;
+          }
+          if (ep.res_mode != 0) {
+            // residual / gate operand at the same pixel and channels, pieces summed smallest first
+            uint32_t w[3] = {0u, 0u, 0u};
+            if (f.valid[hr]) {
+              const uint16_t* src = ep.res.base + f.pix[hr] * ep.res.C + col;
 #pragma unroll
-    for (int pp = 0; pp < 3; ++pp) {
-      const int p = 2 - pp;
-      if (p < planes) {
+              for (int p = 0; p < 3; ++p)
+                if (p < ep.res.planes) w[p] = __ldg(reinterpret_cast<const uint32_t*>(src + p * ep.res.plane));
+            }
+            float r0 = 0.f, r1 = 0.f;
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int idx = it * 32 + c.lane;
-          const int row = idx >> 2, seg = idx & 3;
-          *reinterpret_cast<uint4*>(c.stage + row * 64 + ((seg ^ ((row >> 1) & 3)) << 4)) = q[p][it];
+            for (int pp = 0; pp < 3; ++pp)
+              if (2 - pp < ep.res.planes) add_pair<F16>(w[2 - pp], r0, r1);
+            if (ep.res_mode == 1) { x0 += r0; x1 += r1; }
+            else { x0 *= r0; x1 *= r1; }
+          }
+          if (ep.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
         }
+      }
+      const int col = f.col0 + 32 * ch;
+      for (int p = 0; p < ep.out_planes; ++p) {
+        uint8_t* tile = f.stage + ((f.store_seq++ & 3) << 10);
+        if (f.lane == 0) ptx::bulk_wait_read<3>();      // the store that last used this tile has read it
         __syncwarp();
 #pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-          const uint4 v = *reinterpret_cast<const uint4*>(rowp + ((q4 ^ swz) << 4));
-          const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) add_pair<F16>(w[j], st.r[H * 32 + 8 * q4 + 2 * j], st.r[H * 32 + 8 * q4 + 2 * j + 1]);
-        }
+          for (int hr = 0; hr < 2; ++hr) {
+            const int row = (f.lane >> 2) + 8 * hr;
+            const uint32_t w = split_pair<F16>(x[4 * jj + 2 * hr], x[4 * jj + 2 * hr + 1]);
+            *reinterpret_cast<uint32_t*>(tile + row * 64 + ((jj ^ ((row >> 1) & 3)) << 4) + 4 * q) = w;
+          }
+        ptx::fence_proxy_async_smem();
         __syncwarp();
+        if (f.lane == 0) {
+          if (ep.up2) {
+            const int row0 = f.bn0 * f.g->Ho + f.bh0;   // merged (image, row) coordinate of the 5-D parity view
+#pragma unroll
+            for (int ab = 0; ab < 4; ++ab) ptx::tma_store_5d(&f.maps->c[p], tile, col, ab & 1, f.bw0, ab >> 1, row0);
+          } else if (ep.parity) {
+            ptx::tma_store_5d(&f.maps->c[p], tile, col, (ep.parity - 1) & 1, f.bw0, (ep.parity - 1) >> 1,
+                              f.bn0 * f.g->Ho + f.bh0);
+          } else {
+            ptx::tma_store_4d(&f.maps->c[p], tile, col, f.bw0, f.bh0, f.bn0);
+          }
+          ptx::bulk_commit();
+        }
       }
     }
   }
 
-  // (the residual is loaded inside run(): a per-tile register array kept out of the main loop, where the accumulators live)
+  // fp32 outputs only (ep.out == nullptr; piece outputs take run_frag)
   static __device__ __forceinline__ void prefetch(const Params&, EpiCtx&, State&) {}
-
-  template <int H>
-  static __device__ __forceinline__ void run_half(const Params& ep, const EpiCtx& c, Res& st) {
-    float x[32];
-    const int colt = first_col(c, H);
-    epi_load32<0>(c, colt, x);
-    const int col = c.col0 + colt;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(ep.bias + col) + j);
-      if constexpr (F16) {
-        const float4 sc = __ldg(reinterpret_cast<const float4*>(ep.scale + col) + j);
-        x[4 * j] = fmaf(x[4 * j], sc.x, b.x); x[4 * j + 1] = fmaf(x[4 * j + 1], sc.y, b.y);
-        x[4 * j + 2] = fmaf(x[4 * j + 2], sc.z, b.z); x[4 * j + 3] = fmaf(x[4 * j + 3], sc.w, b.w);
-      } else {
-        x[4 * j] += b.x; x[4 * j + 1] += b.y; x[4 * j + 2] += b.z; x[4 * j + 3] += b.w;
-      }
-    }
-    if (ep.res_mode == 1) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) x[j] += st.r[H * 32 + j];
-    } else if (ep.res_mode == 2) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) x[j] *= st.r[H * 32 + j];
-    }
-    if (ep.relu) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) x[j] = fmaxf(x[j], 0.f);
-    }
-    const int swz = (c.lane >> 1) & 3;
-    for (int p = 0; p < ep.out_planes; ++p) {
-      // the warp's 4 KiB staging area holds two 2 KiB store tiles used alternately: only the store before the previous one
-      // has to have finished reading its tile
-      uint8_t* tile = c.stage + ((c.store_seq++ & 1) << 11);
-      uint8_t* rowp = tile + c.lane * 64;
-      if (c.lane == 0) ptx::bulk_wait_read1();
-      __syncwarp();
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {                   // 16-byte chunks of this row
-        uint32_t w[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) w[j] = split_pair<F16>(x[8 * q + 2 * j], x[8 * q + 2 * j + 1]);
-        *reinterpret_cast<uint4*>(rowp + ((q ^ swz) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
-      ptx::fence_proxy_async_smem();
-      __syncwarp();
-      if (c.lane == 0) {
-        if (ep.up2) {
-          const int row0 = c.bn0 * c.g->Ho + c.bh0;   // merged (image, row) coordinate of the 5-D parity view
-#pragma unroll
-          for (int ab = 0; ab < 4; ++ab) ptx::tma_store_5d(&c.maps->c[p], tile, col, ab & 1, c.bw0, ab >> 1, row0);
-        } else if (ep.parity) {
-          ptx::tma_store_5d(&c.maps->c[p], tile, col, (ep.parity - 1) & 1, c.bw0, (ep.parity - 1) >> 1,
-                            c.bn0 * c.g->Ho + c.bh0);
-        } else {
-          ptx::tma_store_4d(&c.maps->c[p], tile, col, c.bw0, c.bh0, c.bn0);
-        }
-        ptx::bulk_commit();
-      }
-    }
-  }
-
-  static __device__ __forceinline__ void run(const Params& ep, EpiCtx& c, State&) {
-    Res st;
-    if (ep.res_mode != 0 && ep.out != nullptr) {
-      prefetch_half<0>(ep, c, st);
-      if (halves(c) == 2) prefetch_half<1>(ep, c, st);
-    }
-    if (ep.out == nullptr) {
-      run_f32(ep, c);
-    } else if (halves(c) == 2) {
-      run_half<0>(ep, c, st);
-      run_half<1>(ep, c, st);
-    } else {
-      run_half<0>(ep, c, st);
-    }
-  }
+  static __device__ __forceinline__ void run(const Params& ep, EpiCtx& c, State&) { run_f32(ep, c); }
 };
 using EpiConv = EpiConvT<false>;      // bf16 pieces
 using EpiConvH = EpiConvT<true>;      // fp16 hi/lo pieces, per-channel weight scale undone in the epilogue

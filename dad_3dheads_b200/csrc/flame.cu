@@ -214,6 +214,8 @@ flame_prep_kernel(const float* __restrict__ params, int B, FlameLayoutDev L, con
 // ------------------------------------------------------------------------------------------------ K2 epilogue
 struct EpiBlend {
   static constexpr int kExtraSmemBytes = 0;
+  static constexpr int kBf16 = 0;                 // fp16 operands
+  static constexpr bool kFragment = false;        // row epilogue over the shared-memory accumulator tile
   struct State {};
   struct Params {
     float* out;          // [rows, ld] fp32 v_posed * basis_scale (x,y,z interleaved, n = 3*vertex + coord)
@@ -244,6 +246,8 @@ struct EpiBlend {
 // stores are contiguous runs (the reference layout's 60 276-byte row pitch rules out TMA stores).
 struct EpiLbs {
   static constexpr int kExtraSmemBytes = 0;
+  static constexpr int kBf16 = 0;                 // fp16 operands
+  static constexpr bool kFragment = false;        // row epilogue over the shared-memory accumulator tile
   struct Params {
     const float* xf;         // [rows][68] per-head transform records (flame_prep_kernel)
     const float* w2;         // [nv][2]  (w_rest, w_jaw)
@@ -1206,7 +1210,6 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
       g.cl_n = clustered ? 2 : 1;
       g.n_tiles = ceil_div(h->n3, block_n);
       g.block_n = block_n;
-      g.fmt16 = 0;
       if ((flags & DAD3D_BLEND_FAST) && !(flags & DAD3D_BLEND_HILO)) {      // unfused A/B path with one product
         g.nA = 1; g.nB = 1; g.n_mma = 1; g.mma_a[0] = 0; g.mma_b[0] = 0; g.mma_acc[0] = 0; g.n_acc = 1;
       } else {

@@ -185,8 +185,6 @@ __device__ __forceinline__ void tma_store_5d(const void* tmap, const void* smem_
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// all but the most recent bulk group have finished reading their shared-memory source
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 
 // ---------------------------------------------------------------- wgmma (one warpgroup, 128 threads, .sync.aligned)
 // D[64 x N] (fp32, registers) (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory (descriptors below), fp16
@@ -295,6 +293,14 @@ __device__ __forceinline__ void reg_fence(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// per-warpgroup register budget (every warp of the warpgroup executes it); N a multiple of 8 in [24, 256]
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// all but the N most recent bulk groups have finished reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 // named barrier over `threads` threads (id 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");

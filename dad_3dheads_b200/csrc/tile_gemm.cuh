@@ -19,13 +19,18 @@
 // n_mma (6x / 3x).
 //
 // Roles (384 threads = 3 warpgroups): warp 0 = TMA producer (the whole warp walks the schedule, one elect.sync lane issues;
-// warps 1..3 only give their registers back); warpgroups 1 and 2 = consumers: warpgroup w issues the wgmma for tile rows
-// 64w .. 64w+63 (register accumulators), then writes them to a shared-memory accumulator tile and runs the epilogue on
-// them, each thread owning one accumulator row (warp (w, i): rows 32*(2w + i%2) + lane, column group i/2).
+// warps 1..3 only give their registers back: the producer warpgroup drops to kProducerRegs registers per thread and the
+// consumer warpgroups grow to kConsumerRegs); warpgroups 1 and 2 = consumers: warpgroup w issues the wgmma for tile rows
+// 64w .. 64w+63 (register accumulators) and runs the epilogue.  Two epilogue forms, chosen per launch by GemmGeom::frag_epi:
+//   * fragment (frag_epi = 1): each thread works on its own wgmma accumulator registers (warp i of the warpgroup: tile
+//     rows 64w + 16i + lane/4 and +8, column pairs 8j + 2(lane%4)), writes 16-bit results into a swizzled staging tile and
+//     issues TMA stores of its warp's 16 rows x 32 channels.  No shared-memory accumulator tile exists.
+//   * row (frag_epi = 0): the accumulators go to a shared-memory fp32 tile (gemm_acc_bytes) and each thread then owns one
+//     accumulator row (warp (w, i): rows 32*(2w + i%2) + lane, column group i/2) -- for epilogues that need whole rows.
 // Pipeline: smem ring (full/empty mbarriers) between TMA and the consumers; a consumer releases a slot as soon as the
 // wgmma group that read it has completed, so the producer refills it while the next k-block's MMAs run and while the
-// epilogue of a tile runs.  Each epilogue warp owns a 4 KiB shared-memory staging area (two 2 KiB store tiles used
-// alternately) from which it issues TMA stores of its 32 rows x 32 channels.
+// epilogue of a tile runs.  Each epilogue warp owns a 4 KiB shared-memory staging area.
+// The operand format (fp16 / bf16) is Epi::kBf16, a compile-time constant of the epilogue type.
 // Variants selected per launch in GemmGeom: halo (3x3 stride-1 convolutions: one halo patch per channel block feeds all nine
 // taps through shifted descriptors; separate weights ring), res_kb / res_kind (residual or second source on the K axis),
 // cl_m x cl_n multicast clusters.
@@ -42,6 +47,9 @@ constexpr int kMaxMma = 6;
 constexpr int kEpiWarps = 8;
 constexpr int kFirstEpiWarp = 4;
 constexpr int kGemmThreads = (kFirstEpiWarp + kEpiWarps) * 32;   // 384 threads
+// per-role register budgets (setmaxnreg): 128 x 40 + 256 x 232 = 64 512 = the 384 x 168 the launch allocates
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 constexpr int kStageOutBytes = 4096;              // per epilogue warp: 32 rows x 128 B
 constexpr int kGemmSmemLimit = 227 * 1024;
 // halo mode (3x3 stride-1 convolutions): output tiles of 8 x 16 pixels, input halo patch of 10 x 18 pixels per 64-channel
@@ -78,7 +86,8 @@ struct GemmGeom {
   int n_mma_res;                   // products issued for a residual k-block: (mma_res_a[i], B piece 0) -> mma_res_acc[i]
   int mma_res_a[kMaxPieces], mma_res_acc[kMaxPieces];
   int stages;                      // smem ring depth
-  unsigned fmt16;                  // 0 = fp16, 1 = bf16
+  int frag_epi;                    // 1: the epilogue works on the wgmma register fragments (Epi::run_frag) and no fp32
+                                   // accumulator tile is allocated; 0: row epilogue over the shared-memory tile (Epi::run)
   int cl_m, cl_n;                  // thread-block cluster of cl_m x cl_n CTAs (1 or 2 each; plain-GEMM geometry and
                                    // sched 1 only): CTA (ci, cj) of a cluster computes row tile cl_m*Ms+ci, column tile
                                    // cl_n*Ns+cj; the cl_n CTAs sharing a row tile each load 1/cl_n of the A tile and
@@ -112,9 +121,12 @@ __host__ __device__ inline int gemm_stage_bytes(const GemmGeom& g) {
 }
 __host__ __device__ inline int gemm_halo_a_stage_bytes(const GemmGeom& g) { return g.nA * kHaloPieceBytes; }
 __host__ __device__ inline int gemm_b_stage_bytes(const GemmGeom& g) { return g.nB * g.block_n * kBlockK * 2; }
-// shared-memory accumulator tile: 128 rows of gemm_acc_stride floats, 16-byte chunks XOR-swizzled by (row & 7)
+// shared-memory accumulator tile (row epilogues only): 128 rows of gemm_acc_stride floats, 16-byte chunks XOR-swizzled by
+// (row & 7)
 __host__ __device__ inline int gemm_acc_stride(const GemmGeom& g) { return (g.block_n + 31) / 32 * 32; }
-__host__ __device__ inline int gemm_acc_bytes(const GemmGeom& g) { return kBlockM * gemm_acc_stride(g) * 4; }
+__host__ __device__ inline int gemm_acc_bytes(const GemmGeom& g) {
+  return g.frag_epi ? 0 : kBlockM * gemm_acc_stride(g) * 4;
+}
 __host__ inline int gemm_fixed_smem_bytes(const GemmGeom& g, int extra = 0) {
   return kEpiWarps * kStageOutBytes + gemm_acc_bytes(g) + extra + 1024 /*align slack*/ + 512 /*barriers*/;
 }
@@ -179,7 +191,7 @@ __device__ __forceinline__ bool tile_at(const GemmGeom& g, int i, TileCoord* tc)
   return true;
 }
 
-// Everything an epilogue thread needs for one tile.
+// Everything a row-epilogue thread needs for one tile.
 struct EpiCtx {
   const GemmGeom* g;
   const GemmMaps* maps;
@@ -218,6 +230,20 @@ __device__ __forceinline__ void epi_load32(const EpiCtx& c, int c0, float (&x)[N
 // 16 columns [c0, c0+16) into x[OFF..OFF+15]
 template <int OFF, int N>
 __device__ __forceinline__ void epi_load16(const EpiCtx& c, int c0, float (&x)[N]) { epi_load<OFF, 16>(c, c0, x); }
+// Everything a fragment-epilogue thread needs for one tile: its two accumulator rows r0 = 16*wl + lane/4 (within the
+// warpgroup's 64) and r0 + 8, and its warp's 16-row store box.
+struct FragCtx {
+  const GemmGeom* g;
+  const GemmMaps* maps;
+  int lane;
+  uint8_t* stage;        // warp-private 4 KiB staging area: four 1 KiB store tiles used in turn
+  int store_seq;         // number of TMA stores this warp has issued
+  long long pix[2];      // (n*Ho + h)*Wo + w of rows r0, r0 + 8
+  bool valid[2];
+  int col0;              // first output column of the tile
+  int bw0, bh0, bn0;     // the warp's 16-row sub-box origin inside the output tensor
+};
+
 // 32-column chunks [cb, ce) of the tile that column group grp handles
 __device__ __forceinline__ void epi_chunk_range(const GemmGeom& g, int grp, int* cb, int* ce) {
   const int nch = (g.block_n + 31) / 32;          // the last chunk may be 16 columns wide (block_n = 80)
@@ -226,20 +252,16 @@ __device__ __forceinline__ void epi_chunk_range(const GemmGeom& g, int grp, int*
   *ce = min(nch, *cb + per);
 }
 
-// k-steps of one (A piece, B piece) product over a 64-wide k-block into accumulator d
-template <int BN>
-__device__ __forceinline__ void gemm_mma_kblock(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t first,
-                                                unsigned fmt16) {
+// k-steps of one (A piece, B piece) product over a 64-wide k-block into accumulator d (BF16: operand format)
+template <int BN, int BF16>
+__device__ __forceinline__ void gemm_mma_kblock(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t first) {
 #pragma unroll
-  for (int k = 0; k < kBlockK / 16; ++k) {
-    // advancing 16 elements (32 B) along K inside the 128 B swizzle row = +2 in the (addr >> 4) field
-    if (fmt16) ptx::wgmma_m64k16<BN, 1>(d, adesc + 2u * k, bdesc + 2u * k, k > 0 ? 1u : first);
-    else ptx::wgmma_m64k16<BN, 0>(d, adesc + 2u * k, bdesc + 2u * k, k > 0 ? 1u : first);
-  }
+  for (int k = 0; k < kBlockK / 16; ++k)   // 16 elements (32 B) along K inside the 128 B swizzle row = +2 in (addr >> 4)
+    ptx::wgmma_m64k16<BN, BF16>(d, adesc + 2u * k, bdesc + 2u * k, k > 0 ? 1u : first);
 }
 
-// One consumer warpgroup (rows 64*wg ..) over all tiles of this CTA: main loop into registers, accumulator tile to shared
-// memory, epilogue.
+// One consumer warpgroup (rows 64*wg ..) over all tiles of this CTA: main loop into registers, then the fragment epilogue,
+// or the accumulator tile to shared memory and the row epilogue.
 template <class Epi, int BN>
 __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep,
                                               uint8_t* smem, uint8_t* smem_b, float* acc_smem, uint64_t* full_bar,
@@ -264,6 +286,12 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
   float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+  FragCtx f;
+  f.g = &g;
+  f.maps = &maps;
+  f.lane = lane;
+  f.stage = c.stage;
+  f.store_seq = 0;
   typename Epi::State user_state;                // per-thread state that persists across this CTA's tiles
   const int row = c.wq * 32 + lane;
   const int iw = row % g.tw;
@@ -295,8 +323,8 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
             const uint32_t a_id = static_cast<uint32_t>(g.mma_acc[i]);
             const uint32_t first = (started >> a_id) & 1u;
             started |= 1u << a_id;
-            if (a_id) gemm_mma_kblock<BN>(acc1, adesc, bdesc, first, g.fmt16);
-            else gemm_mma_kblock<BN>(acc0, adesc, bdesc, first, g.fmt16);
+            if (a_id) gemm_mma_kblock<BN, Epi::kBf16>(acc1, adesc, bdesc, first);
+            else gemm_mma_kblock<BN, Epi::kBf16>(acc0, adesc, bdesc, first);
           }
           ptx::wgmma_commit();
           ptx::wgmma_wait<1>();                  // the previous group has finished reading its slots
@@ -328,8 +356,8 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
           const uint32_t a_id = static_cast<uint32_t>(res_block ? g.mma_res_acc[i] : g.mma_acc[i]);
           const uint32_t first = (started >> a_id) & 1u;     // 0: this accumulator's first MMA of the tile overwrites
           started |= 1u << a_id;
-          if (a_id) gemm_mma_kblock<BN>(acc1, adesc, bdesc, first, g.fmt16);
-          else gemm_mma_kblock<BN>(acc0, adesc, bdesc, first, g.fmt16);
+          if (a_id) gemm_mma_kblock<BN, Epi::kBf16>(acc1, adesc, bdesc, first);
+          else gemm_mma_kblock<BN, Epi::kBf16>(acc0, adesc, bdesc, first);
         }
         ptx::wgmma_commit();
         if (g.stages == 1) {                     // a one-deep ring: the slot is needed back before the next k-block
@@ -347,6 +375,24 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
     }
     ptx::reg_fence(acc0);
     ptx::reg_fence(acc1);
+    if constexpr (Epi::kFragment) {
+      if (g.frag_epi) {
+        const int row0 = wg * 64 + wl * 16;                   // this warp's 16 tile rows
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = row0 + (lane >> 2) + 8 * hr;
+          const int n = c.tc.n0 + r / (g.tw * g.th), h = c.tc.h0 + (r / g.tw) % g.th, w = c.tc.w0 + r % g.tw;
+          f.valid[hr] = n < g.Nimg && h < g.Ho && w < g.Wo;
+          f.pix[hr] = (static_cast<long long>(n) * g.Ho + h) * g.Wo + w;
+        }
+        f.col0 = c.tc.n_tile * g.block_n;
+        f.bw0 = c.tc.w0 + row0 % g.tw;
+        f.bh0 = c.tc.h0 + (row0 / g.tw) % g.th;
+        f.bn0 = c.tc.n0 + row0 / (g.tw * g.th);
+        Epi::template run_frag<BN>(ep, f, acc0, acc1, g.n_acc == 2);
+        continue;
+      }
+    }
     // ---- accumulator tile (this warpgroup's 64 rows) -> shared memory, then the epilogue reads it row by row
     ptx::bar_sync(1 + wg, 128);                  // every thread of the warpgroup is done with the previous tile's rows
     {
@@ -382,7 +428,7 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
 }
 
 template <class Epi>
-// 12 warps = 3 warpgroups -> at most 168 registers per thread
+// 12 warps = 3 warpgroups -> 168 registers per thread at launch, redistributed by role (kProducerRegs / kConsumerRegs)
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const typename Epi::Params ep) {
   extern __shared__ uint8_t smem_raw[];
@@ -439,130 +485,136 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
   ptx::grid_dep_launch();
   ptx::grid_dep_wait();
 
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    // The WHOLE warp walks the schedule (all control flow and operands stay warp-uniform -> uniform registers); one elected
-    // lane issues the TMA instructions.
-    if (g.halo) {
-      // ---- halo mode: units (tile, channel block) in sequence; the halo patch of unit u+1 is requested while the taps of
-      // unit u are still streaming (after its second tap), the nine weight tiles of a unit follow one another
-      int sa = 0, sbi = 0;
-      uint32_t pha = 0, phb = 0;
-      auto issue_a = [&](const TileCoord& t, int cb) {
-        ptx::mbar_wait(&empty_bar[sa], pha ^ 1u);
-        if (ptx::elect_one_sync()) {
-          ptx::mbar_expect_tx(&full_bar[sa], static_cast<uint32_t>(g.nA * kHaloBytes));
-          for (int i = 0; i < g.nA; ++i)
-            ptx::tma_load_4d(smem + sa * stage_bytes + i * kHaloPieceBytes, &maps.a[i], &full_bar[sa], cb * kBlockK, t.w0 - 1,
-                             t.h0 - 1, t.n0);
-        }
-        __syncwarp();
-        if (++sa == g.stages) { sa = 0; pha ^= 1u; }
-      };
-      int ti = 0, cb = 0;
-      TileCoord tc;
-      bool valid = tile_at(g, 0, &tc);
-      if (valid) issue_a(tc, 0);
-      while (valid) {
-        int nti = ti, ncb = cb + 1;
-        TileCoord ntc = tc;
-        bool nvalid = true;
-        if (ncb == g.cin_blocks) { ncb = 0; ++nti; nvalid = tile_at(g, nti, &ntc); }
-        for (int tap = 0; tap < 9; ++tap) {
-          if (tap == 2 && nvalid) issue_a(ntc, ncb);
-          ptx::mbar_wait(&bempty_bar[sbi], phb ^ 1u);
+  // The register budget changes in the same branch as the role code, so that ptxas allocates each role's code under its
+  // own budget.
+  if (warp < kFirstEpiWarp) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0) {
+      // ===================================================== TMA producer
+      // The WHOLE warp walks the schedule (all control flow and operands stay warp-uniform -> uniform registers); one elected
+      // lane issues the TMA instructions.
+      if (g.halo) {
+        // ---- halo mode: units (tile, channel block) in sequence; the halo patch of unit u+1 is requested while the taps of
+        // unit u are still streaming (after its second tap), the nine weight tiles of a unit follow one another
+        int sa = 0, sbi = 0;
+        uint32_t pha = 0, phb = 0;
+        auto issue_a = [&](const TileCoord& t, int cb) {
+          ptx::mbar_wait(&empty_bar[sa], pha ^ 1u);
           if (ptx::elect_one_sync()) {
-            ptx::mbar_expect_tx(&bfull_bar[sbi], static_cast<uint32_t>(b_stage_bytes));
-            if (csize == 1) {
-              for (int i = 0; i < g.nB; ++i)
-                ptx::tma_load_2d(smem_b + sbi * b_stage_bytes + i * g.block_n * kBlockK * 2, &maps.b[i], &bfull_bar[sbi],
-                                 (tap * g.cin_blocks + cb) * kBlockK, tc.n_tile * g.block_n);
-            } else {
-              // cluster of cl_m row tiles sharing the column tile: I fetch 1/cl_m of the weight rows and multicast them
-              const int b_rows = g.block_n / g.cl_m;
-              for (int i = 0; i < g.nB; ++i)
-                ptx::tma_load_2d_mc(smem_b + sbi * b_stage_bytes + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2,
-                                    &maps.b[i], &bfull_bar[sbi], (tap * g.cin_blocks + cb) * kBlockK,
-                                    tc.n_tile * g.block_n + ci * b_rows, mask_b);
-            }
+            ptx::mbar_expect_tx(&full_bar[sa], static_cast<uint32_t>(g.nA * kHaloBytes));
+            for (int i = 0; i < g.nA; ++i)
+              ptx::tma_load_4d(smem + sa * stage_bytes + i * kHaloPieceBytes, &maps.a[i], &full_bar[sa], cb * kBlockK, t.w0 - 1,
+                               t.h0 - 1, t.n0);
           }
           __syncwarp();
-          if (++sbi == g.stages_b) { sbi = 0; phb ^= 1u; }
+          if (++sa == g.stages) { sa = 0; pha ^= 1u; }
+        };
+        int ti = 0, cb = 0;
+        TileCoord tc;
+        bool valid = tile_at(g, 0, &tc);
+        if (valid) issue_a(tc, 0);
+        while (valid) {
+          int nti = ti, ncb = cb + 1;
+          TileCoord ntc = tc;
+          bool nvalid = true;
+          if (ncb == g.cin_blocks) { ncb = 0; ++nti; nvalid = tile_at(g, nti, &ntc); }
+          for (int tap = 0; tap < 9; ++tap) {
+            if (tap == 2 && nvalid) issue_a(ntc, ncb);
+            ptx::mbar_wait(&bempty_bar[sbi], phb ^ 1u);
+            if (ptx::elect_one_sync()) {
+              ptx::mbar_expect_tx(&bfull_bar[sbi], static_cast<uint32_t>(b_stage_bytes));
+              if (csize == 1) {
+                for (int i = 0; i < g.nB; ++i)
+                  ptx::tma_load_2d(smem_b + sbi * b_stage_bytes + i * g.block_n * kBlockK * 2, &maps.b[i], &bfull_bar[sbi],
+                                   (tap * g.cin_blocks + cb) * kBlockK, tc.n_tile * g.block_n);
+              } else {
+                // cluster of cl_m row tiles sharing the column tile: I fetch 1/cl_m of the weight rows and multicast them
+                const int b_rows = g.block_n / g.cl_m;
+                for (int i = 0; i < g.nB; ++i)
+                  ptx::tma_load_2d_mc(smem_b + sbi * b_stage_bytes + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2,
+                                      &maps.b[i], &bfull_bar[sbi], (tap * g.cin_blocks + cb) * kBlockK,
+                                      tc.n_tile * g.block_n + ci * b_rows, mask_b);
+              }
+            }
+            __syncwarp();
+            if (++sbi == g.stages_b) { sbi = 0; phb ^= 1u; }
+          }
+          ti = nti; cb = ncb; tc = ntc; valid = nvalid;
         }
-        ti = nti; cb = ncb; tc = ntc; valid = nvalid;
-      }
-    } else {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t tx_bytes = static_cast<uint32_t>(stage_bytes);
-      TileCoord tc;
-      for (int ti = 0; tile_at(g, ti, &tc); ++ti) {
-        for (int kb = 0; kb < num_kb + g.res_kb; ++kb) {
-          if (kb >= num_kb) {                      // extra k-blocks fed from the second tensor (maps.r)
+      } else {
+        int stage = 0;
+        uint32_t phase = 0;
+        const uint32_t tx_bytes = static_cast<uint32_t>(stage_bytes);
+        TileCoord tc;
+        for (int ti = 0; tile_at(g, ti, &tc); ++ti) {
+          for (int kb = 0; kb < num_kb + g.res_kb; ++kb) {
+            if (kb >= num_kb) {                      // extra k-blocks fed from the second tensor (maps.r)
+              ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
+              uint8_t* st = smem + stage * stage_bytes;
+              const int r = kb - num_kb;
+              if (ptx::elect_one_sync()) {
+                if (g.res_kind == 0) {
+                  // identity residual: A = residual tile (the tile's own channels), B = identity columns (piece 0 only: the
+                  // other planes are zero there and are never multiplied)
+                  ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(g.nA * kTileABytes + g.block_n * kBlockK * 2));
+                  const int rc = tc.n_tile * g.block_n + r * kBlockK;
+                  for (int i = 0; i < g.nA; ++i)
+                    ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], rc, tc.w0, tc.h0, tc.n0);
+                  ptx::tma_load_2d(st + g.nA * kTileABytes, &maps.b[0], &full_bar[stage], num_kb * kBlockK + rc,
+                                   tc.n_tile * g.block_n);
+                } else {
+                  // second 1x1 source: A = 64 channels of the other tensor at (strided) pixel coordinates, B = its weights
+                  ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
+                  for (int i = 0; i < g.nA; ++i)
+                    ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], r * kBlockK, tc.w0 * g.res_stride,
+                                     tc.h0 * g.res_stride, tc.n0);
+                  uint8_t* sb2 = st + g.nA * kTileABytes;
+                  for (int i = 0; i < g.nB; ++i)
+                    ptx::tma_load_2d(sb2 + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], (num_kb + r) * kBlockK,
+                                     tc.n_tile * g.block_n);
+                }
+              }
+              __syncwarp();
+              if (++stage == g.stages) { stage = 0; phase ^= 1u; }
+              continue;
+            }
+            const int tap = kb / g.cin_blocks;
+            const int cb = kb - tap * g.cin_blocks;
+            const int r = tap / g.S;
+            const int s = tap - r * g.S;
             ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
             uint8_t* st = smem + stage * stage_bytes;
-            const int r = kb - num_kb;
+            const int cw = tc.w0 * g.stride + s - g.pad_w;
+            const int ch = tc.h0 * g.stride + r - g.pad_h;
+            uint8_t* sb = st + g.nA * kTileABytes;
+            const int kcol = kb * kBlockK;
             if (ptx::elect_one_sync()) {
-              if (g.res_kind == 0) {
-                // identity residual: A = residual tile (the tile's own channels), B = identity columns (piece 0 only: the
-                // other planes are zero there and are never multiplied)
-                ptx::mbar_expect_tx(&full_bar[stage], static_cast<uint32_t>(g.nA * kTileABytes + g.block_n * kBlockK * 2));
-                const int rc = tc.n_tile * g.block_n + r * kBlockK;
+              ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
+              if (csize == 1) {
                 for (int i = 0; i < g.nA; ++i)
-                  ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], rc, tc.w0, tc.h0, tc.n0);
-                ptx::tma_load_2d(st + g.nA * kTileABytes, &maps.b[0], &full_bar[stage], num_kb * kBlockK + rc,
-                                 tc.n_tile * g.block_n);
-              } else {
-                // second 1x1 source: A = 64 channels of the other tensor at (strided) pixel coordinates, B = its weights
-                ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
-                for (int i = 0; i < g.nA; ++i)
-                  ptx::tma_load_4d(st + i * kTileABytes, &maps.r[i], &full_bar[stage], r * kBlockK, tc.w0 * g.res_stride,
-                                   tc.h0 * g.res_stride, tc.n0);
-                uint8_t* sb2 = st + g.nA * kTileABytes;
+                  ptx::tma_load_4d(st + i * kTileABytes, &maps.a[i], &full_bar[stage], cb * kBlockK, cw, ch, tc.n0);
                 for (int i = 0; i < g.nB; ++i)
-                  ptx::tma_load_2d(sb2 + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], (num_kb + r) * kBlockK,
+                  ptx::tma_load_2d(sb + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], kcol,
                                    tc.n_tile * g.block_n);
+              } else {
+                // my 1/cl_n slice of the A rows and 1/cl_m slice of the B rows, multicast to the CTAs that share them
+                const int a_rows = kBlockM / g.cl_n, b_rows = g.block_n / g.cl_m;
+                for (int i = 0; i < g.nA; ++i)
+                  ptx::tma_load_4d_mc(st + i * kTileABytes + cj * a_rows * kBlockK * 2, &maps.a[i], &full_bar[stage],
+                                      cb * kBlockK, cw + cj * a_rows, ch, tc.n0, mask_a);
+                for (int i = 0; i < g.nB; ++i)
+                  ptx::tma_load_2d_mc(sb + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2, &maps.b[i],
+                                      &full_bar[stage], kcol, tc.n_tile * g.block_n + ci * b_rows, mask_b);
               }
             }
             __syncwarp();
             if (++stage == g.stages) { stage = 0; phase ^= 1u; }
-            continue;
           }
-          const int tap = kb / g.cin_blocks;
-          const int cb = kb - tap * g.cin_blocks;
-          const int r = tap / g.S;
-          const int s = tap - r * g.S;
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* st = smem + stage * stage_bytes;
-          const int cw = tc.w0 * g.stride + s - g.pad_w;
-          const int ch = tc.h0 * g.stride + r - g.pad_h;
-          uint8_t* sb = st + g.nA * kTileABytes;
-          const int kcol = kb * kBlockK;
-          if (ptx::elect_one_sync()) {
-            ptx::mbar_expect_tx(&full_bar[stage], tx_bytes);
-            if (csize == 1) {
-              for (int i = 0; i < g.nA; ++i)
-                ptx::tma_load_4d(st + i * kTileABytes, &maps.a[i], &full_bar[stage], cb * kBlockK, cw, ch, tc.n0);
-              for (int i = 0; i < g.nB; ++i)
-                ptx::tma_load_2d(sb + i * g.block_n * kBlockK * 2, &maps.b[i], &full_bar[stage], kcol,
-                                 tc.n_tile * g.block_n);
-            } else {
-              // my 1/cl_n slice of the A rows and 1/cl_m slice of the B rows, multicast to the CTAs that share them
-              const int a_rows = kBlockM / g.cl_n, b_rows = g.block_n / g.cl_m;
-              for (int i = 0; i < g.nA; ++i)
-                ptx::tma_load_4d_mc(st + i * kTileABytes + cj * a_rows * kBlockK * 2, &maps.a[i], &full_bar[stage],
-                                    cb * kBlockK, cw + cj * a_rows, ch, tc.n0, mask_a);
-              for (int i = 0; i < g.nB; ++i)
-                ptx::tma_load_2d_mc(sb + i * g.block_n * kBlockK * 2 + ci * b_rows * kBlockK * 2, &maps.b[i],
-                                    &full_bar[stage], kcol, tc.n_tile * g.block_n + ci * b_rows, mask_b);
-            }
-          }
-          __syncwarp();
-          if (++stage == g.stages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp >= kFirstEpiWarp) {
+  } else {
+    ptx::setmaxnreg_inc<kConsumerRegs>();
     // ===================================================== consumer warpgroups: wgmma main loop + epilogue
     const int wg = (warp - kFirstEpiWarp) >> 2;
     const int wl = warp & 3;

@@ -16,8 +16,8 @@ def rows(f):
     d = {}
     for l in open(f):
         p = [x.strip() for x in l.split('|')]
-        if len(p) > 9 and p[1] not in ('layer', '---'):
-            try: d[p[1]] = float(p[8])
+        if len(p) > 10 and p[1] not in ('layer', '---'):
+            try: d[p[1]] = float(p[9])
             except ValueError: pass
     return d
 a, b = rows('gpurun_out/r02_layers_ab_old.md'), rows('gpurun_out/r02_layers_ab_new.md')

@@ -3,11 +3,12 @@
 
 usage: tools/layer_table.py [--batch 64] [--precision fp32] [--reps 7] [--out profiles/r01_layers.md]
 Every row: GEMM shape, device time (median over reps), useful TFLOP/s, executed TFLOP/s (x products per MAC), algorithmic
-GB/s, and the fraction of the larger of its two roofline times (HBM at MEASURED_PEAKS hbm, tensor at bf16 dense)."""
+GB/s, and the fraction of the larger of its two roofline times (HBM and 16-bit dense tensor peaks as bench.py uses them:
+MEASURED_PEAKS.json when present, else the H100 SXM data sheet).  The header records the card, its power limit and SM clock."""
 import argparse
-import json
 import os
 import statistics
+import subprocess
 import sys
 
 import torch
@@ -16,6 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from dad_3dheads_b200.encoder import Dad3dEncoder  # noqa: E402
 from dad_3dheads_b200.encoder_weights import synthetic_state_dict  # noqa: E402
+from bench import _peaks  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=64)
@@ -24,13 +26,19 @@ ap.add_argument("--precision", default="fp32")
 ap.add_argument("--out", default="")
 a = ap.parse_args()
 
-hbm, tens = 6500.0, 1400.0          # GB/s, TFLOP/s fallbacks
-try:
-    pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    hbm = float(pk.get("hbm_gbs", hbm))
-    tens = float(pk.get("bf16_tflops_sustained", tens))
-except Exception:
-    pass
+pk = _peaks()
+hbm, tens = float(pk["hbm_gbs"]), float(pk["bf16_tflops_sustained"])   # GB/s, TFLOP/s
+
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", "--id=0", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=20).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        out = ""
+    return out or "unknown (nvidia-smi unavailable)"
+
 
 dev = torch.device("cuda", 0)
 enc = Dad3dEncoder(synthetic_state_dict(0), dev, precision=a.precision, want_heatmap=False)
@@ -38,6 +46,7 @@ x = torch.randn(a.batch, 3, 256, 256, device=dev)
 for _ in range(3):
     enc.forward_raw(x)
 torch.cuda.synchronize()
+gpu_before = card()
 runs = []
 for _ in range(a.reps):
     enc.set_profile(True)
@@ -46,6 +55,7 @@ for _ in range(a.reps):
     runs.append(enc.profile_layers())
     enc.profile_read()
 enc.set_profile(False)
+gpu_after = card()
 rows = []
 for i, r in enumerate(runs[0]):
     r = dict(r)
@@ -54,15 +64,17 @@ for i, r in enumerate(runs[0]):
 tot = sum(r["ms"] for r in rows)
 lines = [f"# encoder tile-engine launches, batch {a.batch}, precision {a.precision}: {len(rows)} launches, {tot * 1e3:.0f} us "
          f"(median of {a.reps} forwards, CUDA events around each launch, so launch gaps are excluded)", "",
-         f"roofline denominators: HBM {hbm:.0f} GB/s, bf16 dense {tens:.0f} TFLOP/s; `frac` = max(bytes/HBM, executed flops/tensor) / time", "",
-         "| layer | M | K | N | kblk | tiles | stg | us | useful TF/s | exec TF/s | GB/s | t_hbm us | t_mma us | frac |",
-         "|---|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
+         f"GPU (name, power limit, SM clock, max SM clock) before / after the timed forwards: {gpu_before} / {gpu_after}", "",
+         f"roofline denominators ({pk['source']}): HBM {hbm:.0f} GB/s, 16-bit dense {tens:.0f} TFLOP/s; "
+         "`frac` = max(bytes/HBM, executed flops/tensor) / time", "",
+         "| layer | M | K | N | bn | kblk | tiles | stg | us | useful TF/s | exec TF/s | GB/s | t_hbm us | t_mma us | frac |",
+         "|---|---|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
 for r in rows:
     us = r["ms"] * 1e3
     ex = r["flops"] * r["products"]
     t_h = r["bytes"] / (hbm * 1e9) * 1e6
     t_m = ex / (tens * 1e12) * 1e6
-    lines.append(f"| {r['name']} | {r['M']} | {r['K']} | {r['N']} | {r['k_blocks']} | {r['tiles']} | {r['stages']} | {us:.1f} | "
+    lines.append(f"| {r['name']} | {r['M']} | {r['K']} | {r['N']} | {r['block_n']} | {r['k_blocks']} | {r['tiles']} | {r['stages']} | {us:.1f} | "
                  f"{r['flops'] / us / 1e6:.0f} | {ex / us / 1e6:.0f} | {r['bytes'] / us / 1e3:.0f} | {t_h:.1f} | {t_m:.1f} | "
                  f"{max(t_h, t_m) / us:.2f} |")
 ideal = sum(max(r["bytes"] / (hbm * 1e9), r["flops"] * r["products"] / (tens * 1e12)) for r in rows) * 1e6
