@@ -80,6 +80,10 @@ SIGNATURES = {
     "dad3d_encoder_set_debug": (C.c_int, [C.c_void_p, C.c_int32]),
     "dad3d_encoder_read_activation": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t,
                                                  C.POINTER(C.c_int32), C.c_void_p]),
+    "dad3d_encoder_describe_plan": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    "dad3d_encoder_write_activation": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_encoder_run_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p]),
 }
 
 

@@ -710,6 +710,110 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
   return DAD3D_OK;
 }
 
+// one step of the plan, as dad3d_encoder_forward runs it (the single-step test hook runs the same code)
+int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* params_d, float* landmarks_d, float* heatmap_d,
+             cudaStream_t stream) {
+  const Plan& plan = *enc->plan;
+  const int B = plan.B;
+  auto T = [&](int id) -> const TensorInfo& { return plan.tensors[id]; };
+  auto view = [&](int id) {
+    const TensorInfo& t = T(id);
+    return ActView{reinterpret_cast<const uint16_t*>(t.ptr), t.plane_elems(), t.planes, t.C, enc->fp16};
+  };
+  switch (s.kind) {
+    case kStemConv: {
+      const TensorInfo& to = T(s.out_f32);
+      dim3 grid(ceil_div(to.W, kStemTile), ceil_div(to.H, kStemTile), B);
+      if (!enc->stem_configured) {
+        DAD3D_CUDA_OK(cudaFuncSetAttribute(stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStemSmemBytes));
+        enc->stem_configured = true;
+      }
+      stem_conv_kernel<<<grid, 256, kStemSmemBytes, stream>>>(images_d, enc->d_stem_w, enc->d_stem_b, kImg, kImg,
+                                                 reinterpret_cast<float*>(to.ptr));
+      count_launch();
+      break;
+    }
+    case kStemS2d: {
+      const TensorInfo& to = T(s.out);
+      stem_s2d_kernel<<<dim3(static_cast<unsigned>(ceil_div(to.W, 128)), static_cast<unsigned>(to.H), static_cast<unsigned>(B)),
+                        128, 0, stream>>>(
+          images_d, B, kImg, kImg, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes, enc->fp16);
+      count_launch();
+      break;
+    }
+    case kStemPool: {
+      const TensorInfo& ti = T(s.in);
+      const TensorInfo& to = T(s.out);
+      ActView pieces{nullptr, 0, 0, 0, enc->fp16};
+      if (!ti.f32) pieces = view(s.in);
+      const long long total = static_cast<long long>(B) * to.H * to.W * 8;
+      DAD3D_REQUIRE(total < (1ll << 31), "pool: batch too large for 32-bit indexing");
+      stem_pool_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+          reinterpret_cast<const float*>(ti.ptr), pieces, B, ti.H, ti.W, reinterpret_cast<uint16_t*>(to.ptr),
+          to.plane_elems(), to.planes, enc->fp16);
+      count_launch();
+      break;
+    }
+    case kConv: {
+      if ((s.variant == 1 && !heatmap_d) || (s.variant == 2 && heatmap_d)) break;     // heat-map head: full map / support rows
+      int rc = launch_conv(enc, s, stream);
+      if (rc != DAD3D_OK) return rc;
+      break;
+    }
+    case kFuse: {
+      const TensorInfo& to = T(s.out);
+      FuseSrc f0{view(s.in), T(s.in).H, T(s.in).W, s.fw[0]};
+      FuseSrc f1{view(s.in2), T(s.in2).H, T(s.in2).W, s.fw[1]};
+      FuseSrc f2 = f1;
+      if (s.nsrc == 3) f2 = FuseSrc{view(s.in3), T(s.in3).H, T(s.in3).W, s.fw[2]};
+      const dim3 fgrid(static_cast<unsigned>(ceil_div(to.W * (to.C / 8), 256)), static_cast<unsigned>(to.H),
+                       static_cast<unsigned>(to.N));
+      bifpn_fuse_kernel<<<fgrid, 256, 0, stream>>>(
+          f0, f1, f2, s.nsrc, to.N, to.H, to.W, to.C, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes,
+          enc->fp16);
+      count_launch();
+      break;
+    }
+    case kConcat: {
+      const TensorInfo& to = T(s.out);
+      const TensorInfo& th = T(s.in2);
+      const int cthreads = ceil_div(to.C / 8, 32) * 32;
+      DAD3D_REQUIRE(cthreads <= 1024, "concat: too many channels");
+      fusion_concat_kernel<<<dim3(static_cast<unsigned>(to.H * to.W), static_cast<unsigned>(to.N)), cthreads, 0, stream>>>(
+          view(s.in), T(s.in).C, reinterpret_cast<const float*>(th.ptr), th.H, th.W, th.C, kHeat, kHeatCat, view(s.in3),
+          T(s.in3).C, to.N, to.H, to.W, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes, enc->fp16);
+      count_launch();
+      break;
+    }
+    case kGap: {
+      const TensorInfo& ti = T(s.in);
+      const TensorInfo& to = T(s.out);
+      gap_kernel<<<B * (ti.C / 64), 256, 0, stream>>>(view(s.in), B, ti.H * ti.W, ti.C,
+                                                           reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes,
+                                                           enc->fp16);
+      count_launch();
+      break;
+    }
+    case kFinalize: {
+      const TensorInfo& ti = T(s.in);
+      head_finalize_kernel<<<ceil_div(B * kMlpOut, 256), 256, 0, stream>>>(reinterpret_cast<const float*>(ti.ptr), ti.C, B,
+                                                                          kLimitValue, params_d, landmarks_d);
+      count_launch();
+      break;
+    }
+    case kHeatExport: {
+      if (!heatmap_d) break;
+      const TensorInfo& ti = T(s.in);
+      const long long total = static_cast<long long>(B) * kHeat * ti.H * ti.W;
+      heatmap_export_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+          reinterpret_cast<const float*>(ti.ptr), ti.C, B, ti.H * ti.W, kHeat, heatmap_d);
+      count_launch();
+      break;
+    }
+  }
+  return DAD3D_OK;
+}
+
 }  // namespace
 
 // =================================================================================================== C ABI
@@ -933,104 +1037,9 @@ int dad3d_encoder_forward(dad3d_encoder* enc, const float* images_d, int32_t B, 
     int rc = make_plan(enc, B, workspace_d, workspace_bytes, false, nullptr);
     if (rc != DAD3D_OK) return rc;
   }
-  const Plan& plan = *enc->plan;
-  auto T = [&](int id) -> const TensorInfo& { return plan.tensors[id]; };
-  auto view = [&](int id) {
-    const TensorInfo& t = T(id);
-    return ActView{reinterpret_cast<const uint16_t*>(t.ptr), t.plane_elems(), t.planes, t.C, enc->fp16};
-  };
-  for (const Step& s : plan.steps) {
-    switch (s.kind) {
-      case kStemConv: {
-        const TensorInfo& to = T(s.out_f32);
-        dim3 grid(ceil_div(to.W, kStemTile), ceil_div(to.H, kStemTile), B);
-        if (!enc->stem_configured) {
-          DAD3D_CUDA_OK(cudaFuncSetAttribute(stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStemSmemBytes));
-          enc->stem_configured = true;
-        }
-        stem_conv_kernel<<<grid, 256, kStemSmemBytes, stream>>>(images_d, enc->d_stem_w, enc->d_stem_b, kImg, kImg,
-                                                   reinterpret_cast<float*>(to.ptr));
-        count_launch();
-        break;
-      }
-      case kStemS2d: {
-        const TensorInfo& to = T(s.out);
-        stem_s2d_kernel<<<dim3(static_cast<unsigned>(ceil_div(to.W, 128)), static_cast<unsigned>(to.H), static_cast<unsigned>(B)),
-                          128, 0, stream>>>(
-            images_d, B, kImg, kImg, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes, enc->fp16);
-        count_launch();
-        break;
-      }
-      case kStemPool: {
-        const TensorInfo& ti = T(s.in);
-        const TensorInfo& to = T(s.out);
-        ActView pieces{nullptr, 0, 0, 0, enc->fp16};
-        if (!ti.f32) pieces = view(s.in);
-        const long long total = static_cast<long long>(B) * to.H * to.W * 8;
-        DAD3D_REQUIRE(total < (1ll << 31), "pool: batch too large for 32-bit indexing");
-        stem_pool_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
-            reinterpret_cast<const float*>(ti.ptr), pieces, B, ti.H, ti.W, reinterpret_cast<uint16_t*>(to.ptr),
-            to.plane_elems(), to.planes, enc->fp16);
-        count_launch();
-        break;
-      }
-      case kConv: {
-        if ((s.variant == 1 && !heatmap_d) || (s.variant == 2 && heatmap_d)) break;     // heat-map head: full map / support rows
-        int rc = launch_conv(enc, s, stream);
-        if (rc != DAD3D_OK) return rc;
-        break;
-      }
-      case kFuse: {
-        const TensorInfo& to = T(s.out);
-        FuseSrc f0{view(s.in), T(s.in).H, T(s.in).W, s.fw[0]};
-        FuseSrc f1{view(s.in2), T(s.in2).H, T(s.in2).W, s.fw[1]};
-        FuseSrc f2 = f1;
-        if (s.nsrc == 3) f2 = FuseSrc{view(s.in3), T(s.in3).H, T(s.in3).W, s.fw[2]};
-        const dim3 fgrid(static_cast<unsigned>(ceil_div(to.W * (to.C / 8), 256)), static_cast<unsigned>(to.H),
-                         static_cast<unsigned>(to.N));
-        bifpn_fuse_kernel<<<fgrid, 256, 0, stream>>>(
-            f0, f1, f2, s.nsrc, to.N, to.H, to.W, to.C, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes,
-            enc->fp16);
-        count_launch();
-        break;
-      }
-      case kConcat: {
-        const TensorInfo& to = T(s.out);
-        const TensorInfo& th = T(s.in2);
-        const int cthreads = ceil_div(to.C / 8, 32) * 32;
-        DAD3D_REQUIRE(cthreads <= 1024, "concat: too many channels");
-        fusion_concat_kernel<<<dim3(static_cast<unsigned>(to.H * to.W), static_cast<unsigned>(to.N)), cthreads, 0, stream>>>(
-            view(s.in), T(s.in).C, reinterpret_cast<const float*>(th.ptr), th.H, th.W, th.C, kHeat, kHeatCat, view(s.in3),
-            T(s.in3).C, to.N, to.H, to.W, reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes, enc->fp16);
-        count_launch();
-        break;
-      }
-      case kGap: {
-        const TensorInfo& ti = T(s.in);
-        const TensorInfo& to = T(s.out);
-        gap_kernel<<<B * (ti.C / 64), 256, 0, stream>>>(view(s.in), B, ti.H * ti.W, ti.C,
-                                                             reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes,
-                                                             enc->fp16);
-        count_launch();
-        break;
-      }
-      case kFinalize: {
-        const TensorInfo& ti = T(s.in);
-        head_finalize_kernel<<<ceil_div(B * kMlpOut, 256), 256, 0, stream>>>(reinterpret_cast<const float*>(ti.ptr), ti.C, B,
-                                                                            kLimitValue, params_d, landmarks_d);
-        count_launch();
-        break;
-      }
-      case kHeatExport: {
-        if (!heatmap_d) break;
-        const TensorInfo& ti = T(s.in);
-        const long long total = static_cast<long long>(B) * kHeat * ti.H * ti.W;
-        heatmap_export_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
-            reinterpret_cast<const float*>(ti.ptr), ti.C, B, ti.H * ti.W, kHeat, heatmap_d);
-        count_launch();
-        break;
-      }
-    }
+  for (const Step& s : enc->plan->steps) {
+    int rc = run_step(enc, s, images_d, params_d, landmarks_d, heatmap_d, stream);
+    if (rc != DAD3D_OK) return rc;
   }
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
@@ -1133,6 +1142,102 @@ int dad3d_encoder_read_activation(dad3d_encoder* enc, const char* name, float* o
   }
   set_error(std::string("no activation named ") + name);
   return DAD3D_ERR_INVALID;
+}
+
+int dad3d_encoder_describe_plan(dad3d_encoder* enc, char* buf, size_t cap) {
+  DAD3D_REQUIRE(enc && buf, "null pointer");
+  DAD3D_REQUIRE(enc->plan, "no forward has run yet");
+  static const char* kKinds[] = {"stem_conv", "stem_s2d", "stem_pool", "conv", "fuse", "concat", "gap", "finalize",
+                                 "heat_export"};
+  const Plan& plan = *enc->plan;
+  std::string j = "{\"B\":" + std::to_string(plan.B) + ",\"pieces\":" + std::to_string(enc->P) +
+                  ",\"fp16\":" + std::to_string(enc->fp16) + ",\"num_sms\":" + std::to_string(enc->num_sms) + ",\"steps\":[";
+  auto num = [&](const char* k, long long v) { j += "\""; j += k; j += "\":" + std::to_string(v) + ","; };
+  auto tensor = [&](const char* k, int id) {
+    if (id < 0) return;
+    const TensorInfo& t = plan.tensors[id];
+    j += "\""; j += k;
+    j += "\":{\"name\":\"" + t.name + "\",\"N\":" + std::to_string(t.N) + ",\"H\":" + std::to_string(t.H) +
+         ",\"W\":" + std::to_string(t.W) + ",\"C\":" + std::to_string(t.C) + ",\"planes\":" + std::to_string(t.planes) +
+         ",\"f32\":" + (t.f32 ? "true" : "false") + "},";
+  };
+  for (size_t i = 0; i < plan.steps.size(); ++i) {
+    const Step& s = plan.steps[i];
+    j += i ? ",{" : "{";
+    j += "\"kind\":\"" + std::string(kKinds[s.kind]) + "\",\"layer\":\"" + (s.w ? s.w->name : std::string()) + "\",";
+    num("variant", s.variant);
+    tensor("in", s.in); tensor("in2", s.in2); tensor("in3", s.in3); tensor("res", s.res); tensor("out", s.out);
+    tensor("out_f32", s.out_f32);
+    if (s.kind == kFuse) j += "\"fw\":[" + std::to_string(s.fw[0]) + "," + std::to_string(s.fw[1]) + "," +
+                              std::to_string(s.fw[2]) + "],";
+    if (s.kind == kConv) {
+      const GemmGeom& g = s.geom;
+      num("stride", s.stride); num("pad", s.pad); num("relu", s.relu); num("res_mode", s.res_mode); num("stem", s.stem);
+      num("R", g.R); num("S", g.S);
+      num("tw", g.tw); num("th", g.th); num("tn", g.tn); num("tiles_w", g.tiles_w); num("tiles_h", g.tiles_h);
+      num("tiles_n", g.tiles_n); num("block_n", g.block_n); num("n_tiles", g.n_tiles); num("stages", g.stages);
+      num("stages_b", g.stages_b); num("halo", g.halo); num("cl_m", g.cl_m); num("cl_n", g.cl_n); num("sched", g.sched);
+      num("frag_epi", g.frag_epi); num("res_kb", g.res_kb); num("res_kind", g.res_kind); num("res_stride", g.res_stride);
+      num("up2", s.up2); num("parity", s.parity); num("rowmap_n", g.rowmap_n); num("n_mma", g.n_mma); num("n_acc", g.n_acc);
+      num("cout", s.w->cout); num("cin", s.w->cin); num("has_identity", s.w->has_identity ? 1 : 0);
+      j += "\"rowmap\":[";
+      for (int r = 0; r < g.rowmap_n; ++r) j += (r ? "," : "") + std::to_string(g.rowmap[r]);
+      j += "],";
+    }
+    j.back() = '}';
+  }
+  j += "]}";
+  if (j.size() + 1 > cap) {
+    set_error("plan description needs " + std::to_string(j.size() + 1) + " bytes");
+    return DAD3D_ERR_INVALID;
+  }
+  std::memcpy(buf, j.c_str(), j.size() + 1);
+  return DAD3D_OK;
+}
+
+int dad3d_encoder_write_activation(dad3d_encoder* enc, const char* name, const float* src_d, size_t n, dad3d_stream stream_) {
+  DAD3D_REQUIRE(enc && name && src_d, "null pointer");
+  DAD3D_REQUIRE(enc->plan && enc->plan->ws, "no forward has run yet");
+  // without keep_all, tensors whose lifetimes do not overlap share workspace: a write would clobber live activations
+  DAD3D_REQUIRE(enc->debug_keep_all, "write_activation needs dad3d_encoder_set_debug(enc, 1)");
+  for (const TensorInfo& t : enc->plan->tensors) {
+    if (t.name != name) continue;
+    const size_t elems = static_cast<size_t>(t.plane_elems());
+    DAD3D_REQUIRE(n == elems, "write_activation: element count does not match the tensor");
+    DAD3D_REQUIRE(t.ptr, "write_activation: tensor has no storage");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    if (t.f32) {
+      DAD3D_CUDA_OK(cudaMemcpyAsync(t.ptr, src_d, n * 4, cudaMemcpyDeviceToDevice, stream));
+    } else {
+      DAD3D_REQUIRE(t.C % 8 == 0, "write_activation: channel count not a multiple of 8");
+      const long long n8 = static_cast<long long>(n / 8);
+      f32_to_pieces_kernel<<<static_cast<unsigned>((n8 + 255) / 256), 256, 0, stream>>>(
+          src_d, n8, reinterpret_cast<uint16_t*>(t.ptr), t.plane_elems(), t.planes, enc->fp16);
+      count_launch();
+      DAD3D_CUDA_OK(cudaGetLastError());
+    }
+    return DAD3D_OK;
+  }
+  set_error(std::string("no activation named ") + name);
+  return DAD3D_ERR_INVALID;
+}
+
+int dad3d_encoder_run_steps(dad3d_encoder* enc, int32_t first, int32_t count, const float* images_d, float* params_d,
+                            float* landmarks_d, float* heatmap_d, dad3d_stream stream_) {
+  DAD3D_REQUIRE(enc, "null handle");
+  DAD3D_REQUIRE(enc->plan && enc->plan->ws, "no plan: run a forward at this batch size and workspace first");
+  const int n = static_cast<int>(enc->plan->steps.size());
+  DAD3D_REQUIRE(first >= 0 && count >= 0 && first + count <= n, "step range outside the plan");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  for (int i = first; i < first + count; ++i) {
+    const Step& s = enc->plan->steps[i];
+    DAD3D_REQUIRE(images_d || (s.kind != kStemConv && s.kind != kStemS2d), "this step reads the images");
+    DAD3D_REQUIRE((params_d && landmarks_d) || s.kind != kFinalize, "this step writes params and landmarks");
+    int rc = run_step(enc, s, images_d, params_d, landmarks_d, heatmap_d, stream);
+    if (rc != DAD3D_OK) return rc;
+  }
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
 }
 
 int dad3d_encoder_num_layers(const dad3d_encoder* enc) { return enc ? static_cast<int>(enc->convs.size()) : 0; }   // "stem" is in convs too

@@ -563,6 +563,16 @@ __global__ void pieces_to_f32_kernel(ActView a, long long n, float* __restrict__
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) out[i] = act_load(a, i);
 }
+// test hook: split fp32 values into the piece planes (n8 groups of 8 consecutive elements), the split every kernel stores
+__global__ void f32_to_pieces_kernel(const float* __restrict__ in, long long n8, uint16_t* __restrict__ base,
+                                     long long plane, int planes, int fp16) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n8) return;
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = in[i * 8 + j];
+  act_store8(base, plane, planes, fp16, i * 8, v);
+}
 
 // heat-map NHWC fp32 [B,HW,ld] -> NCHW fp32 [B,68,HW] (the reference's OUTPUT_LANDMARKS_HEATMAP layout)
 __global__ void heatmap_export_kernel(const float* __restrict__ in, int ld, int B, int HW, int C,

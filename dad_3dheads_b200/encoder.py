@@ -147,6 +147,10 @@ class Dad3dEncoder:
 
     def __init__(self, state_dict: Dict[str, Tensor], device: Optional[torch.device] = None, precision: str = "fp32",
                  want_heatmap: bool = True):
+        self._setup(device, precision, want_heatmap)
+        self._create(*fold_state_dict(state_dict))
+
+    def _setup(self, device, precision, want_heatmap):
         if not torch.cuda.is_available():
             raise _lib.Dad3dError("dad_3dheads_b200 needs a CUDA (sm_90a) device: there is no CPU path")
         self.lib = _lib.load()
@@ -155,8 +159,21 @@ class Dad3dEncoder:
             raise _lib.Dad3dError(f"Dad3dEncoder needs a cuda device, got {self.device}")
         self.precision = precision
         self.want_heatmap = want_heatmap
-        pieces, fmt = PRECISION_PIECES[precision], PRECISION_FORMAT[precision]
-        layers, fusion_w = fold_state_dict(state_dict)
+
+    @classmethod
+    def from_folded(cls, layers: List[Tuple[str, np.ndarray, np.ndarray]], fusion_w: np.ndarray,
+                    device: Optional[torch.device] = None, precision: str = "fp32", want_heatmap: bool = True):
+        """An encoder over already folded layer records (the output format of :func:`fold_state_dict`), no BN folding:
+        tests hand designed weights straight to dad3d_encoder_create."""
+        enc = cls.__new__(cls)
+        enc._setup(device, precision, want_heatmap)
+        enc._create(layers, np.ascontiguousarray(fusion_w, dtype=np.float32))
+        return enc
+
+    def _create(self, layers, fusion_w):
+        pieces, fmt = PRECISION_PIECES[self.precision], PRECISION_FORMAT[self.precision]
+        layers = [(n, np.ascontiguousarray(w, dtype=np.float32), np.ascontiguousarray(b, dtype=np.float32))
+                  for n, w, b in layers]
         recs = (_ConvWeights * len(layers))()
         keep = []
         for i, (name, w, b) in enumerate(layers):
@@ -225,6 +242,34 @@ class Dad3dEncoder:
                                                               torch.cuda.current_stream(self.device).cuda_stream),
                        "dad3d_encoder_read_activation")
         return out
+
+    def describe_plan(self) -> dict:
+        """The plan of the last forward: {"B", "pieces", "fp16", "num_sms", "steps": [per step: kind, layer, variant, the
+        tensors it touches (in / in2 / in3 / res / out / out_f32 with name, N, H, W, C, planes, f32) and, for conv steps,
+        the tile-engine geometry]}."""
+        import json
+        buf = C.create_string_buffer(1 << 20)
+        _lib.check(self.lib.dad3d_encoder_describe_plan(self._h, buf, len(buf)), "dad3d_encoder_describe_plan")
+        return json.loads(buf.value.decode())
+
+    def write_activation(self, name: str, x: Tensor) -> None:
+        """Overwrite activation ``name`` of the current plan with fp32 NHWC ``x`` (channels padded as stored), split into
+        pieces by the library's own split."""
+        x = x.to(self.device, torch.float32).contiguous()
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.dad3d_encoder_write_activation(self._h, name.encode(), x.data_ptr(), x.numel(),
+                                                               torch.cuda.current_stream(self.device).cuda_stream),
+                       "dad3d_encoder_write_activation")
+
+    def run_steps(self, first: int, count: int = 1, images: Optional[Tensor] = None, params: Optional[Tensor] = None,
+                  landmarks: Optional[Tensor] = None, heatmap: Optional[Tensor] = None) -> None:
+        """Run steps [first, first + count) of the current plan, exactly as the forward runs them (``heatmap`` selects the
+        heat-map variants as in the forward)."""
+        ptr = lambda t: t.data_ptr() if t is not None else None     # noqa: E731
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.dad3d_encoder_run_steps(self._h, first, count, ptr(images), ptr(params), ptr(landmarks),
+                                                        ptr(heatmap), torch.cuda.current_stream(self.device).cuda_stream),
+                       "dad3d_encoder_run_steps")
 
     def forward_raw(self, x: Tensor, want_heatmap: Optional[bool] = None):
         """x: [B,3,256,256] fp32 CUDA.  -> (params [B,413], landmarks [B,68,2], heatmap [B,68,64,64] | None)."""

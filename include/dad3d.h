@@ -188,6 +188,20 @@ DAD3D_API int dad3d_encoder_profile_layer(dad3d_encoder* enc, int32_t index, cha
 DAD3D_API int dad3d_encoder_set_debug(dad3d_encoder* enc, int32_t keep_all);
 DAD3D_API int dad3d_encoder_read_activation(dad3d_encoder* enc, const char* name, float* out_d, size_t capacity_floats,
                                             int32_t* dims4, dad3d_stream stream);
+/* test hooks for single-step checks of the current plan (the one the last forward built):
+ *   describe_plan  writes a NUL-terminated JSON description of every step (kind, layer, variant, the tensors it reads and
+ *                  writes with their extents, and the tile-engine geometry of conv steps) into buf[cap]
+ *   write_activation  the inverse of read_activation: src_d is fp32 NHWC [N,H,W,C] with channels padded as stored, n its
+ *                  element count (must equal the tensor's); piece tensors are split with the library's own RN split, fp32
+ *                  tensors are copied raw.  Only with keep_all on (set_debug), where no two tensors share workspace;
+ *                  otherwise it fails
+ *   run_steps      runs steps [first, first + count) of the plan exactly as dad3d_encoder_forward would (same launches,
+ *                  same variant selection by heatmap_d); B and the workspace are those of the plan */
+DAD3D_API int dad3d_encoder_describe_plan(dad3d_encoder* enc, char* buf, size_t cap);
+DAD3D_API int dad3d_encoder_write_activation(dad3d_encoder* enc, const char* name, const float* src_d, size_t n,
+                                             dad3d_stream stream);
+DAD3D_API int dad3d_encoder_run_steps(dad3d_encoder* enc, int32_t first, int32_t count, const float* images_d,
+                                      float* params_d, float* landmarks_d, float* heatmap_d, dad3d_stream stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Benchmark evaluator hot spots (SURVEY §8f row 1; dad_3dheads_benchmark/benchmark.py, dad_3dheads_benchmark/utils.py),
