@@ -42,6 +42,11 @@ SIGNATURES = {
     "dad3d_flame_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
     "dad3d_flame_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float,
                                       C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_flame_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_int32, C.c_void_p]),
+    "dad3d_flame_decode_from": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                           C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_flame_describe": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_char_p, C.c_size_t]),
     "dad3d_flame_backward_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
     "dad3d_flame_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float,
                                         C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

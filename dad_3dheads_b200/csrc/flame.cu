@@ -354,15 +354,15 @@ struct EpiLbs {
         if (ep.proj) {
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            const float qx = ((x[3 * i] * st.sc + st.tx) + 1.0f) * 0.5f * ep.image_size;       // head_mesh.py:40-43
-            const float qy = ((x[3 * i + 1] * st.sc + st.ty) + 1.0f) * 0.5f * ep.image_size;
+            const float qx = (fmaf(x[3 * i], st.sc, st.tx) + 1.0f) * 0.5f * ep.image_size;       // head_mesh.py:40-43
+            const float qy = (fmaf(x[3 * i + 1], st.sc, st.ty) + 1.0f) * 0.5f * ep.image_size;
             if (ep.pc == 2) {
               stage[c.lane * 25 + 2 * i] = qx;
               stage[c.lane * 25 + 2 * i + 1] = qy;
             } else {
               stage[c.lane * 25 + 3 * i] = qx;
               stage[c.lane * 25 + 3 * i + 1] = qy;
-              stage[c.lane * 25 + 3 * i + 2] = ((x[3 * i + 2] * st.sc + 0.0f) + 1.0f) * 0.5f * ep.image_size;
+              stage[c.lane * 25 + 3 * i + 2] = (fmaf(x[3 * i + 2], st.sc, 0.0f) + 1.0f) * 0.5f * ep.image_size;
             }
           }
           if (ep.pc == 2)
@@ -437,11 +437,11 @@ lbs_project_kernel(const float* __restrict__ vposed, int ldv, const float* __res
       s_out[3 * t + 1] = oy;
       s_out[3 * t + 2] = oz;
       const float sc = s_xf[63];
-      const float px = ((ox * sc + s_xf[64]) + 1.0f) * 0.5f * image_size;     // head_mesh.py:40-43
-      const float py = ((oy * sc + s_xf[65]) + 1.0f) * 0.5f * image_size;
+      const float px = (fmaf(ox, sc, s_xf[64]) + 1.0f) * 0.5f * image_size;     // head_mesh.py:40-43
+      const float py = (fmaf(oy, sc, s_xf[65]) + 1.0f) * 0.5f * image_size;
       s_proj[pc * t] = px;
       s_proj[pc * t + 1] = py;
-      if (pc == 3) s_proj[3 * t + 2] = ((oz * sc + 0.0f) + 1.0f) * 0.5f * image_size;
+      if (pc == 3) s_proj[3 * t + 2] = (fmaf(oz, sc, 0.0f) + 1.0f) * 0.5f * image_size;
     }
     __syncthreads();
     if (verts3d) {
@@ -810,9 +810,10 @@ struct dad3d_flame {
 
 namespace {
 
+// Launch configuration of one tile-engine launch: grid size (CTAs) in *grid.  Shared by the launch and dad3d_flame_describe.
 template <class Epi>
-int launch_tile_gemm(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep, int num_sms,
-                     cudaStream_t stream, int* configured, int* max_clusters_cache) {
+int tile_gemm_config(const GemmGeom& g, int num_sms, int* configured, int* max_clusters_cache, cudaLaunchConfig_t* cfg,
+                     cudaLaunchAttribute* attr) {
   // function attributes are per device: remembered in the handle, not in a process-wide static
   const int smem = gemm_smem_bytes(g, Epi::kExtraSmemBytes);
   if (!*configured) {
@@ -821,36 +822,61 @@ int launch_tile_gemm(const GemmMaps& maps, const GemmGeom& g, const typename Epi
   }
   const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
   const int csize = g.cl_m * g.cl_n;
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
-  cfg.numAttrs = 0;
+  *cfg = cudaLaunchConfig_t{};
+  cfg->blockDim = dim3(kGemmThreads);
+  cfg->dynamicSmemBytes = smem;
+  cfg->attrs = attr;
+  cfg->numAttrs = 0;
   if (csize > 1) {
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = csize;
     attr[0].val.clusterDim.y = 1;
     attr[0].val.clusterDim.z = 1;
-    cfg.numAttrs = 1;
+    cfg->numAttrs = 1;
     int& max_clusters = *max_clusters_cache;           // co-resident clusters of this size (GPC packing: < #SM / csize);
     if (max_clusters == 0) {                           // cached in the handle: occupancy is a per-device property
-      cfg.gridDim = dim3(num_sms / csize * csize);
-      DAD3D_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, tile_gemm_kernel<Epi>, &cfg));
+      cfg->gridDim = dim3(num_sms / csize * csize);
+      DAD3D_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, tile_gemm_kernel<Epi>, cfg));
       if (max_clusters < 1) { set_error("no co-resident cluster fits"); return DAD3D_ERR_CUDA; }
     }
     const int m_super = ceil_div(m_tiles, g.cl_m);
     const int clusters = m_super < max_clusters ? m_super : max_clusters;
-    cfg.gridDim = dim3(clusters * csize);
+    cfg->gridDim = dim3(clusters * csize);
   } else {
     const int total = g.sched == 1 ? m_tiles : m_tiles * g.n_tiles;
-    cfg.gridDim = dim3(total < num_sms ? total : num_sms);
+    cfg->gridDim = dim3(total < num_sms ? total : num_sms);
   }
+  return DAD3D_OK;
+}
+
+template <class Epi>
+int launch_tile_gemm(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep, int num_sms,
+                     cudaStream_t stream, int* configured, int* max_clusters_cache) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  const int rc = tile_gemm_config<Epi>(g, num_sms, configured, max_clusters_cache, &cfg, attr);
+  if (rc != DAD3D_OK) return rc;
+  cfg.stream = stream;
   DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<Epi>, maps, g, ep));
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
+}
+
+// Schedule of one flame_decode_kernel launch over `rows` heads: fills rows, nv, n_tiles, m_units, splits and stages of *p and
+// returns the grid size (CTAs).  Shared by the launch and dad3d_flame_describe.
+int dec_schedule(const dad3d_flame* h, int rows, DecodeParams* p) {
+  p->rows = rows;
+  p->nv = h->nv;
+  p->n_tiles = ceil_div(h->n3, kDecN);
+  p->m_units = dec_rows_padded(rows) / kDecBlockM;                // whole permutation blocks: two row tiles per 256 heads
+  const int groups_max = h->num_sms;
+  // fewer row tiles than SMs: split every row tile's sweep over the vertex tiles so that all SMs get work
+  p->splits = p->m_units >= groups_max ? 1 : ceil_div(groups_max, p->m_units);
+  if (p->splits > p->n_tiles) p->splits = p->n_tiles;
+  const int units = p->m_units * p->splits;
+  p->stages = dec_max_stages();
+  return units < groups_max ? units : groups_max;
 }
 
 // One launch of flame_decode_kernel over `rows` heads whose fp16 coefficient rows (a_hi) and transform records (xf) the prep
@@ -870,17 +896,7 @@ int launch_flame_decode(dad3d_flame* h, const __half* a_hi, int rows, const floa
     if (!make_tmap_16bit(&map_a, a_hi, 2, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
   }
   DecodeParams p;
-  p.rows = rows;
-  p.nv = h->nv;
-  p.n_tiles = ceil_div(h->n3, kDecN);
-  p.m_units = dec_rows_padded(rows) / kDecBlockM;                  // whole permutation blocks: two row tiles per 256 heads
-  const int groups_max = h->num_sms;
-  // fewer row tiles than SMs: split every row tile's sweep over the vertex tiles so that all SMs get work
-  p.splits = p.m_units >= groups_max ? 1 : ceil_div(groups_max, p.m_units);
-  if (p.splits > p.n_tiles) p.splits = p.n_tiles;
-  const int units = p.m_units * p.splits;
-  const int groups = units < groups_max ? units : groups_max;
-  p.stages = dec_max_stages();
+  const int groups = dec_schedule(h, rows, &p);
   if (p.stages < 2) { set_error("decode pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
   p.xf = xf;
   p.w2 = h->d_w2p;
@@ -1004,7 +1020,8 @@ int dad3d_flame_create(dad3d_flame** out, const float* shapedirs_h, const float*
     }
     // template: two columns with coefficient 1 (kTmplCol, kTmplCol+1 -- the prep kernel writes 1.0 into both).  The
     // successive fp16 pieces p0..p3 of scale*T go to (col0.hi, col1.hi, col0.lo, col1.lo): the hi planes alone already
-    // carry 22 bits (what the one-product FAST mode sees), all four planes are exact in fp32.
+    // carry 22 bits (what the one-product FAST mode sees), all four planes are exact in fp32 unless the last piece underflows
+    // fp16 (then within 2^-25).
     float r = v_template_h[n] * h->basis_scale;
     unsigned short pc[4];
     for (int k = 0; k < 4; ++k) {
@@ -1139,6 +1156,110 @@ size_t dad3d_flame_workspace_bytes(const dad3d_flame* h, int32_t B) {
   return unfused > fused ? unfused : fused;
 }
 
+// The four decode paths.  Default: the dedicated one-product decode kernel (flame_decode.cuh); DAD3D_BLEND_HILO = 3-product hi/lo
+// operands through the tile engine with the fused EpiLbs epilogue (fp32-class blend product); general layouts and
+// DAD3D_DECODE_UNFUSED: EpiBlend to a v_posed scratch + lbs_project_kernel; DAD3D_BLEND_SIMT: CUDA-core product +
+// lbs_project_kernel.  DAD3D_BLEND_FAST is the old name of today's default and is accepted as a no-op.
+enum DecodePath { kPathDedicated, kPathLbs, kPathBlend, kPathSimt };
+static DecodePath decode_path(const dad3d_flame* h, int flags) {
+  const bool fused = h->jaw_only && !(flags & (DAD3D_BLEND_SIMT | DAD3D_DECODE_UNFUSED));
+  if (fused) return (flags & DAD3D_BLEND_HILO) ? kPathLbs : kPathDedicated;
+  return (flags & DAD3D_BLEND_SIMT) ? kPathSimt : kPathBlend;
+}
+static bool path_fused(DecodePath path) { return path == kPathDedicated || path == kPathLbs; }
+// heads per pass: the fused paths need no v_posed scratch
+static int decode_chunk(const dad3d_flame* h, DecodePath path) { return path_fused(path) ? h->fused_chunk : kDecodeChunk; }
+// big fused passes (>= one row tile per SM): 2x2 thread-block clusters with TMA multicast of both operands (opt-in)
+static bool decode_clustered(const dad3d_flame* h, DecodePath path, int rows, int flags) {
+  return path == kPathLbs && ceil_div(rows, kBlockM) >= h->num_sms && (flags & DAD3D_DECODE_CLUSTER);
+}
+
+// Tile-engine geometry of the blend product of one pass (kPathLbs / kPathBlend)
+static GemmGeom blend_geom(const dad3d_flame* h, DecodePath path, int rows, int flags) {
+  const bool fused = path == kPathLbs;
+  const bool clustered = decode_clustered(h, path, rows, flags);
+  const int block_n = fused ? kFusedBlockN : kBlendBlockN;
+  GemmGeom g;
+  std::memset(&g, 0, sizeof(g));
+  g.tw = kBlockM; g.th = 1; g.tn = 1;
+  g.tiles_w = ceil_div(rows, kBlockM); g.tiles_h = 1; g.tiles_n = 1;
+  g.Wo = rows; g.Ho = 1; g.Nimg = 1;
+  g.stride = 1; g.R = 1; g.S = 1; g.pad_h = 0; g.pad_w = 0;
+  g.cin_blocks = kKPad / kBlockK;
+  g.cl_m = clustered ? 2 : 1;
+  g.cl_n = clustered ? 2 : 1;
+  g.n_tiles = ceil_div(h->n3, block_n);
+  g.block_n = block_n;
+  if ((flags & DAD3D_BLEND_FAST) && !(flags & DAD3D_BLEND_HILO)) {      // unfused A/B path with one product
+    g.nA = 1; g.nB = 1; g.n_mma = 1; g.mma_a[0] = 0; g.mma_b[0] = 0; g.mma_acc[0] = 0; g.n_acc = 1;
+  } else {
+    g.nA = 2; g.nB = 2; g.n_mma = 3; g.n_acc = 2;
+    g.mma_a[0] = 1; g.mma_b[0] = 0; g.mma_acc[0] = 1;   // lo*hi, hi*lo: small terms, own accumulator
+    g.mma_a[1] = 0; g.mma_b[1] = 1; g.mma_acc[1] = 1;
+    g.mma_a[2] = 0; g.mma_b[2] = 0; g.mma_acc[2] = 0;   // hi*hi
+  }
+  if (fused) {
+    g.sched = g.tiles_w >= h->num_sms ? 1 : 0;          // enough row tiles to give every SM its own
+    g.stages = gemm_max_stages(g, EpiLbs::kExtraSmemBytes);
+  } else {
+    g.sched = 0;
+    g.stages = gemm_max_stages(g);
+  }
+  return g;
+}
+
+// K1 alone: coefficient rows (permuted for the dedicated kernel) and transform records of `rows` heads
+static int flame_prep(dad3d_flame* h, const float* p, int rows, int flags, __half* a_hi, __half* a_lo, float* xf, bool permute,
+                      cudaStream_t stream) {
+  const int threads = 256;
+  const int group = rows >= 32 * 8 * h->num_sms ? 32 : 1;              // heads per warp (see the kernel)
+  const int blocks = ceil_div(ceil_div(rows, group) * 32, threads);
+  flame_prep_kernel<<<blocks, threads, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags, 1.0f / h->basis_scale, a_hi,
+                                                    a_lo, xf, permute ? 1 : 0, group);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+// Everything after K1 for one pass of `rows` <= decode_chunk heads: the product and skinning of the path `flags` selects
+static int flame_decode_stage(dad3d_flame* h, const __half* a_hi, const __half* a_lo, const float* xf, int rows, int flags,
+                              float* v3, float* pj, int pc, float image_size, float* vposed, cudaStream_t stream) {
+  const DecodePath path = decode_path(h, flags);
+  if (path == kPathDedicated) return launch_flame_decode(h, a_hi, rows, xf, v3, pj, pc, image_size, stream);
+  if (path == kPathSimt) {
+    dim3 grid(ceil_div(h->npad, 256), rows);
+    blend_simt_kernel<<<grid, 256, 0, stream>>>(a_hi, a_lo, h->d_basis[0], h->d_basis[1], rows, h->npad, vposed);
+    count_launch();
+    DAD3D_CUDA_OK(cudaGetLastError());
+  } else {
+    const bool clustered = decode_clustered(h, path, rows, flags);
+    GemmMaps maps;
+    std::memset(&maps, 0, sizeof(maps));
+    const __half* planes[2] = {a_hi, a_lo};
+    for (int pi = 0; pi < 2; ++pi) {
+      const uint64_t dims[4] = {static_cast<uint64_t>(kKPad), static_cast<uint64_t>(rows), 1, 1};
+      const uint64_t strides[3] = {static_cast<uint64_t>(kKPad) * 2, static_cast<uint64_t>(kKPad) * 2 * rows,
+                                   static_cast<uint64_t>(kKPad) * 2 * rows};
+      const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(clustered ? kBlockM / 2 : kBlockM), 1, 1};
+      if (!make_tmap_16bit(&maps.a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
+      maps.b[pi] = path == kPathLbs ? (clustered ? h->map_b48[pi] : h->map_b96[pi]) : h->map_b[pi];
+    }
+    const GemmGeom g = blend_geom(h, path, rows, flags);
+    if (path == kPathLbs) {
+      EpiLbs::Params ep{xf, h->d_w2, h->nv, v3, pj, pc, image_size};
+      return launch_tile_gemm<EpiLbs>(maps, g, ep, h->num_sms, stream, &h->smem_configured[0], &h->max_clusters[0]);
+    }
+    EpiBlend::Params ep{vposed, h->npad};
+    int rc = launch_tile_gemm<EpiBlend>(maps, g, ep, h->num_sms, stream, &h->smem_configured[1], &h->max_clusters[0]);
+    if (rc != DAD3D_OK) return rc;
+  }
+  dim3 grid(ceil_div(h->nv, kLbsThreads), rows < 1024 ? rows : 1024);
+  lbs_project_kernel<<<grid, kLbsThreads, 0, stream>>>(vposed, h->npad, h->d_weights, xf, rows, h->nv, v3, pj, pc, image_size);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
 int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, float* vertices3d_d,
                        float* projected_d, float image_size, int32_t to_2d, void* workspace_d, size_t workspace_bytes,
                        dad3d_stream stream_) {
@@ -1148,11 +1269,8 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
   DAD3D_REQUIRE(vertices3d_d || projected_d, "at least one output must be requested");
   DAD3D_REQUIRE(workspace_d && workspace_bytes >= dad3d_flame_workspace_bytes(h, B), "workspace too small");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const bool fused = h->jaw_only && !(flags & (DAD3D_BLEND_SIMT | DAD3D_DECODE_UNFUSED));
-  // default: the dedicated one-product decode kernel (flame_decode.cuh); DAD3D_BLEND_HILO = 3-product hi/lo operands through
-  // the tile engine (fp32-class blend product).  DAD3D_BLEND_FAST is the old name of today's default and is accepted as a no-op.
-  const bool dedicated = fused && !(flags & DAD3D_BLEND_HILO);
-  const int chunk = fused ? h->fused_chunk : kDecodeChunk;
+  const DecodePath path = decode_path(h, flags);
+  const int chunk = decode_chunk(h, path);
   const int rows_max = B < chunk ? B : chunk;
   uint8_t* ws = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<uintptr_t>(workspace_d), 1024));
   __half* a_hi = reinterpret_cast<__half*>(ws);
@@ -1160,86 +1278,93 @@ int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t B, int32_t
   float* xf = reinterpret_cast<float*>(ws + 2 * ws_coef_bytes(rows_max));
   float* vposed = reinterpret_cast<float*>(ws + 2 * ws_coef_bytes(rows_max) + ws_xf_bytes(rows_max));
   const int pc = to_2d ? 2 : 3;
-  const float inv_scale = 1.0f / h->basis_scale;
 
   for (int b0 = 0; b0 < B; b0 += chunk) {
     const int rows = (B - b0) < chunk ? (B - b0) : chunk;
     const float* p = params_d + static_cast<size_t>(b0) * h->layout.n_params;
     float* v3 = vertices3d_d ? vertices3d_d + static_cast<size_t>(b0) * h->nv * 3 : nullptr;
     float* pj = projected_d ? projected_d + static_cast<size_t>(b0) * h->nv * pc : nullptr;
-    {
-      const int threads = 256;
-      const int group = rows >= 32 * 8 * h->num_sms ? 32 : 1;              // heads per warp (see the kernel)
-      const int blocks = ceil_div(ceil_div(rows, group) * 32, threads);
-      flame_prep_kernel<<<blocks, threads, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags, inv_scale, a_hi,
-                                                        a_lo, xf, dedicated ? 1 : 0, group);
-      count_launch();
-      DAD3D_CUDA_OK(cudaGetLastError());
-    }
-    if (dedicated) {
-      int rc = launch_flame_decode(h, a_hi, rows, xf, v3, pj, pc, image_size, stream);
-      if (rc != DAD3D_OK) return rc;
-    } else if (flags & DAD3D_BLEND_SIMT) {
-      dim3 grid(ceil_div(h->npad, 256), rows);
-      blend_simt_kernel<<<grid, 256, 0, stream>>>(a_hi, a_lo, h->d_basis[0], h->d_basis[1], rows, h->npad, vposed);
-      count_launch();
-      DAD3D_CUDA_OK(cudaGetLastError());
-    } else {
-      const int block_n = fused ? kFusedBlockN : kBlendBlockN;
-      // big fused passes (>= one row tile per SM): 2x2 thread-block clusters with TMA multicast of both operands (opt-in)
-      const bool clustered = fused && ceil_div(rows, kBlockM) >= h->num_sms && (flags & DAD3D_DECODE_CLUSTER);
-      GemmMaps maps;
-      std::memset(&maps, 0, sizeof(maps));
-      __half* planes[2] = {a_hi, a_lo};
-      for (int pi = 0; pi < 2; ++pi) {
-        const uint64_t dims[4] = {static_cast<uint64_t>(kKPad), static_cast<uint64_t>(rows), 1, 1};
-        const uint64_t strides[3] = {static_cast<uint64_t>(kKPad) * 2, static_cast<uint64_t>(kKPad) * 2 * rows,
-                                     static_cast<uint64_t>(kKPad) * 2 * rows};
-        const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(clustered ? kBlockM / 2 : kBlockM), 1, 1};
-        if (!make_tmap_16bit(&maps.a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
-        maps.b[pi] = fused ? (clustered ? h->map_b48[pi] : h->map_b96[pi]) : h->map_b[pi];
-      }
-      GemmGeom g;
-      std::memset(&g, 0, sizeof(g));
-      g.tw = kBlockM; g.th = 1; g.tn = 1;
-      g.tiles_w = ceil_div(rows, kBlockM); g.tiles_h = 1; g.tiles_n = 1;
-      g.Wo = rows; g.Ho = 1; g.Nimg = 1;
-      g.stride = 1; g.R = 1; g.S = 1; g.pad_h = 0; g.pad_w = 0;
-      g.cin_blocks = kKPad / kBlockK;
-      g.cl_m = clustered ? 2 : 1;
-      g.cl_n = clustered ? 2 : 1;
-      g.n_tiles = ceil_div(h->n3, block_n);
-      g.block_n = block_n;
-      if ((flags & DAD3D_BLEND_FAST) && !(flags & DAD3D_BLEND_HILO)) {      // unfused A/B path with one product
-        g.nA = 1; g.nB = 1; g.n_mma = 1; g.mma_a[0] = 0; g.mma_b[0] = 0; g.mma_acc[0] = 0; g.n_acc = 1;
-      } else {
-        g.nA = 2; g.nB = 2; g.n_mma = 3; g.n_acc = 2;
-        g.mma_a[0] = 1; g.mma_b[0] = 0; g.mma_acc[0] = 1;   // lo*hi, hi*lo: small terms, own accumulator
-        g.mma_a[1] = 0; g.mma_b[1] = 1; g.mma_acc[1] = 1;
-        g.mma_a[2] = 0; g.mma_b[2] = 0; g.mma_acc[2] = 0;   // hi*hi
-      }
-      if (fused) {
-        g.sched = g.tiles_w >= h->num_sms ? 1 : 0;          // enough row tiles to give every SM its own
-        g.stages = gemm_max_stages(g, EpiLbs::kExtraSmemBytes);
-        EpiLbs::Params ep{xf, h->d_w2, h->nv, v3, pj, pc, image_size};
-        int rc = launch_tile_gemm<EpiLbs>(maps, g, ep, h->num_sms, stream, &h->smem_configured[0], &h->max_clusters[0]);
-        if (rc != DAD3D_OK) return rc;
-      } else {
-        g.sched = 0;
-        g.stages = gemm_max_stages(g);
-        EpiBlend::Params ep{vposed, h->npad};
-        int rc = launch_tile_gemm<EpiBlend>(maps, g, ep, h->num_sms, stream, &h->smem_configured[1], &h->max_clusters[0]);
-        if (rc != DAD3D_OK) return rc;
-      }
-    }
-    if (!fused) {
-      dim3 grid(ceil_div(h->nv, kLbsThreads), rows < 1024 ? rows : 1024);
-      lbs_project_kernel<<<grid, kLbsThreads, 0, stream>>>(vposed, h->npad, h->d_weights, xf, rows, h->nv, v3, pj, pc,
-                                                           image_size);
-      count_launch();
-      DAD3D_CUDA_OK(cudaGetLastError());
-    }
+    int rc = flame_prep(h, p, rows, flags, a_hi, a_lo, xf, path == kPathDedicated, stream);
+    if (rc != DAD3D_OK) return rc;
+    rc = flame_decode_stage(h, a_hi, a_lo, xf, rows, flags, v3, pj, pc, image_size, vposed, stream);
+    if (rc != DAD3D_OK) return rc;
   }
+  return DAD3D_OK;
+}
+
+int dad3d_flame_prep(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, void* coef_hi_d, void* coef_lo_d,
+                     float* xf_d, int32_t permute, dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && params_d && coef_hi_d && coef_lo_d && xf_d, "null pointer");
+  return flame_prep(h, params_d, B, flags, static_cast<__half*>(coef_hi_d), static_cast<__half*>(coef_lo_d), xf_d, permute != 0,
+                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_flame_decode_from(dad3d_flame* h, const void* coef_hi_d, const void* coef_lo_d, const float* xf_d, int32_t B,
+                            int32_t flags, float* vertices3d_d, float* projected_d, float image_size, int32_t to_2d,
+                            void* workspace_d, size_t workspace_bytes, dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && coef_hi_d && coef_lo_d && xf_d, "null pointer");
+  DAD3D_REQUIRE(vertices3d_d || projected_d, "at least one output must be requested");
+  const DecodePath path = decode_path(h, flags);
+  DAD3D_REQUIRE(B <= decode_chunk(h, path), "B exceeds one pass of the selected decode path");
+  float* vposed = nullptr;
+  if (!path_fused(path)) {
+    DAD3D_REQUIRE(workspace_d && workspace_bytes >= ws_vposed_bytes(h, B) + 1024, "workspace too small");
+    vposed = reinterpret_cast<float*>(align_up(reinterpret_cast<uintptr_t>(workspace_d), 1024));
+  }
+  return flame_decode_stage(h, static_cast<const __half*>(coef_hi_d), static_cast<const __half*>(coef_lo_d), xf_d, B, flags,
+                            vertices3d_d, projected_d, to_2d ? 2 : 3, image_size, vposed, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_flame_describe(dad3d_flame* h, int32_t B, int32_t flags, char* json, size_t cap) {
+  DAD3D_REQUIRE(h && json && cap > 0, "null pointer");
+  DAD3D_REQUIRE(B >= 0, "B");
+  const DecodePath path = decode_path(h, flags);
+  const int chunk = decode_chunk(h, path);
+  static const char* kNames[4] = {"dedicated", "lbs", "blend", "simt"};
+  char scale[32];
+  std::snprintf(scale, sizeof(scale), "%.17g", static_cast<double>(h->basis_scale));
+  std::string out = "{\"basis_scale\": " + std::string(scale) + ", \"jaw_only\": " + (h->jaw_only ? "true" : "false") +
+                    ", \"nv\": " + std::to_string(h->nv) + ", \"npad\": " + std::to_string(h->npad) +
+                    ", \"fused_chunk\": " + std::to_string(h->fused_chunk) + ", \"num_sms\": " + std::to_string(h->num_sms) +
+                    ", \"passes\": [";
+  for (int b0 = 0; b0 < B; b0 += chunk) {
+    const int rows = (B - b0) < chunk ? (B - b0) : chunk;
+    int m_units = 0, splits = 1, grid = 0, stages = 0;
+    bool clustered = false;
+    if (path == kPathDedicated) {
+      DecodeParams p;
+      grid = dec_schedule(h, rows, &p);
+      m_units = p.m_units;
+      splits = p.splits;
+      stages = p.stages;
+    } else if (path == kPathSimt) {
+      m_units = rows;
+      grid = ceil_div(h->npad, 256) * rows;
+    } else {
+      const GemmGeom g = blend_geom(h, path, rows, flags);
+      cudaLaunchConfig_t cfg;
+      cudaLaunchAttribute attr[1];
+      int rc = path == kPathLbs
+                   ? tile_gemm_config<EpiLbs>(g, h->num_sms, &h->smem_configured[0], &h->max_clusters[0], &cfg, attr)
+                   : tile_gemm_config<EpiBlend>(g, h->num_sms, &h->smem_configured[1], &h->max_clusters[0], &cfg, attr);
+      if (rc != DAD3D_OK) return rc;
+      m_units = g.tiles_w;
+      grid = static_cast<int>(cfg.gridDim.x);
+      stages = g.stages;
+      clustered = g.cl_m * g.cl_n > 1;
+    }
+    out += std::string(b0 ? ", " : "") + "{\"path\": \"" + kNames[path] + "\", \"rows\": " + std::to_string(rows) +
+           ", \"m_units\": " + std::to_string(m_units) + ", \"splits\": " + std::to_string(splits) +
+           ", \"grid\": " + std::to_string(grid) + ", \"stages\": " + std::to_string(stages) +
+           ", \"clustered\": " + (clustered ? "true" : "false") + "}";
+  }
+  out += "]}";
+  DAD3D_REQUIRE(out.size() < cap, "json buffer too small");
+  std::memcpy(json, out.c_str(), out.size() + 1);
   return DAD3D_OK;
 }
 

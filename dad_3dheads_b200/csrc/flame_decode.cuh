@@ -342,14 +342,14 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
             if (pc == 2) {
 #pragma unroll
               for (int i = 0; i < 4; ++i) {
-                qcar[2 * i] = ((xpre[3 * i] * sc + tx) + 1.0f) * hs;
-                qcar[2 * i + 1] = ((xpre[3 * i + 1] * sc + ty) + 1.0f) * hs;
+                qcar[2 * i] = (fmaf(xpre[3 * i], sc, tx) + 1.0f) * hs;
+                qcar[2 * i + 1] = (fmaf(xpre[3 * i + 1], sc, ty) + 1.0f) * hs;
               }
             } else {
 #pragma unroll
               for (int j = 0; j < 8; ++j) {
                 const int e = 4 + j;                 // float e of the 12: coordinate e % 3
-                qcar[j] = ((xpre[e] * sc + (e % 3 == 0 ? tx : e % 3 == 1 ? ty : 0.0f)) + 1.0f) * hs;
+                qcar[j] = (fmaf(xpre[e], sc, e % 3 == 0 ? tx : e % 3 == 1 ? ty : 0.0f) + 1.0f) * hs;
               }
             }
           }
@@ -382,8 +382,8 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
                 float qv[16];
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
-                  qv[2 * i] = ((x[3 * i] * sc + tx) + 1.0f) * hs;
-                  qv[2 * i + 1] = ((x[3 * i + 1] * sc + ty) + 1.0f) * hs;
+                  qv[2 * i] = (fmaf(x[3 * i], sc, tx) + 1.0f) * hs;
+                  qv[2 * i + 1] = (fmaf(x[3 * i + 1], sc, ty) + 1.0f) * hs;
                 }
                 if (row_ok) {
                   if (ncols >= kDecPassCols) dec_store<16>(q_row + vfirst * 2, c_q, qcar, qv, first, last);
@@ -395,9 +395,9 @@ flame_decode_kernel(const __grid_constant__ CUtensorMap map_a,     // coefficien
                 float qv[24];
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
-                  qv[3 * i] = ((x[3 * i] * sc + tx) + 1.0f) * hs;
-                  qv[3 * i + 1] = ((x[3 * i + 1] * sc + ty) + 1.0f) * hs;
-                  qv[3 * i + 2] = ((x[3 * i + 2] * sc + 0.0f) + 1.0f) * hs;
+                  qv[3 * i] = (fmaf(x[3 * i], sc, tx) + 1.0f) * hs;
+                  qv[3 * i + 1] = (fmaf(x[3 * i + 1], sc, ty) + 1.0f) * hs;
+                  qv[3 * i + 2] = (fmaf(x[3 * i + 2], sc, 0.0f) + 1.0f) * hs;
                 }
                 if (row_ok) {
                   if (ncols >= kDecPassCols) dec_store<24>(q_row + col0, c_q, qcar, qv, first, last);

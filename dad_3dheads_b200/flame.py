@@ -179,6 +179,69 @@ class FlameDecoder:
                                                    stream), "dad3d_flame_decode")
         return v3, pj
 
+    # ---- test hooks: the two stages of a decode pass on caller buffers (include/dad3d.h)
+    def describe(self, B: int, flags: int = 0) -> Dict[str, Any]:
+        """Packing constants and, per pass of a decode of ``B`` heads with ``flags``, the launch the library would make."""
+        import json
+        buf = C.create_string_buffer(1 << 16)
+        _lib.check(self.lib.dad3d_flame_describe(self._h, int(B), int(flags), buf, len(buf)), "dad3d_flame_describe")
+        return json.loads(buf.value.decode())
+
+    def prep(self, params: Tensor, *, flags: int = 0, permute: bool = False):
+        """flame_prep_kernel alone: (coef_hi, coef_lo) [B rounded up to 256, 448] fp16 (padding rows unwritten: zeros here)
+        and the [B, 68] transform records."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.shape[1] == self.num_params
+        params = params.contiguous()
+        B = params.shape[0]
+        rows = (B + 255) // 256 * 256
+        hi = torch.zeros(rows, 448, dtype=torch.float16, device=params.device)
+        lo = torch.zeros_like(hi)
+        xf = torch.empty(B, 68, dtype=torch.float32, device=params.device)
+        with torch.cuda.device(params.device):
+            _lib.check(self.lib.dad3d_flame_prep(self._h, params.data_ptr(), B, int(flags), hi.data_ptr(), lo.data_ptr(),
+                                                 xf.data_ptr(), 1 if permute else 0,
+                                                 torch.cuda.current_stream(params.device).cuda_stream), "dad3d_flame_prep")
+        return hi, lo, xf
+
+    def decode_from(self, coef_hi: Tensor, coef_lo: Tensor, xf: Tensor, *, flags: int = 0, vertices: Optional[Tensor] = None,
+                    projected: Optional[Tensor] = None, image_size: float = 256.0, to_2d: bool = True) -> None:
+        """The stage after prep for one pass of ``xf.shape[0]`` heads, written into the caller's ``vertices`` [B,V,3] /
+        ``projected`` [B,V,2|3] views (either may be None).  Rows are permuted for the dedicated kernel only."""
+        B = xf.shape[0]
+        for t in (coef_hi, coef_lo):
+            assert t.dtype == torch.float16 and t.is_contiguous() and t.shape[1] == 448 and t.shape[0] >= (B + 255) // 256 * 256
+        assert xf.dtype == torch.float32 and xf.is_contiguous() and xf.shape == (B, 68)
+        self._check_out(vertices, B, 3)
+        self._check_out(projected, B, 2 if to_2d else 3)
+        nbytes = int(self.lib.dad3d_flame_workspace_bytes(self._h, B))
+        ws = self._ws.get(xf.device, nbytes)
+        with torch.cuda.device(xf.device):
+            _lib.check(self.lib.dad3d_flame_decode_from(
+                self._h, coef_hi.data_ptr(), coef_lo.data_ptr(), xf.data_ptr(), B, int(flags),
+                vertices.data_ptr() if vertices is not None else None, projected.data_ptr() if projected is not None else None,
+                float(image_size), 1 if to_2d else 0, ws.data_ptr(), ws.numel(),
+                torch.cuda.current_stream(xf.device).cuda_stream), "dad3d_flame_decode_from")
+
+    def decode_into(self, params: Tensor, *, flags: int = 0, vertices: Optional[Tensor] = None,
+                    projected: Optional[Tensor] = None, image_size: float = 256.0, to_2d: bool = True) -> None:
+        """``dad3d_flame_decode`` into caller-owned output views (``decode`` allocates its own): for guard-band tests."""
+        assert params.is_cuda and params.dtype == torch.float32 and params.shape[1] == self.num_params
+        params = params.contiguous()
+        B = params.shape[0]
+        self._check_out(vertices, B, 3)
+        self._check_out(projected, B, 2 if to_2d else 3)
+        nbytes = int(self.lib.dad3d_flame_workspace_bytes(self._h, B))
+        ws = self._ws.get(params.device, nbytes)
+        with torch.cuda.device(params.device):
+            _lib.check(self.lib.dad3d_flame_decode(
+                self._h, params.data_ptr(), B, int(flags), vertices.data_ptr() if vertices is not None else None,
+                projected.data_ptr() if projected is not None else None, float(image_size), 1 if to_2d else 0,
+                ws.data_ptr(), ws.numel(), torch.cuda.current_stream(params.device).cuda_stream), "dad3d_flame_decode")
+
+    def _check_out(self, t: Optional[Tensor], B: int, nc: int) -> None:
+        if t is not None:
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == (B, self.n_vertices, nc), t.shape
+
     def backward(self, params: Tensor, grad_vertices: Optional[Tensor], grad_projected: Optional[Tensor], *, to_2d: bool = True,
                  zero_rot: bool = False, zero_jaw: bool = False, image_size: float = 256.0) -> Tensor:
         """d L / d params [B, num_params] from d L / d vertices3d [B,V,3] and / or d L / d projected [B,V,2|3] (either may be

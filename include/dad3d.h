@@ -87,6 +87,27 @@ DAD3D_API int dad3d_flame_decode(dad3d_flame* h, const float* params_d, int32_t 
                        float* projected_d, float image_size, int32_t to_2d, void* workspace_d, size_t workspace_bytes,
                        dad3d_stream stream);
 
+/* test hooks: the two stages of every decode pass, run alone on caller buffers (dad3d_flame_decode runs each pass as
+ * dad3d_flame_prep followed by dad3d_flame_decode_from, 2 kernel launches on the fused paths and 3 on the others)
+ *   dad3d_flame_prep   flame_prep_kernel alone: coef_hi_d / coef_lo_d [dec_rows_padded(B) = B rounded up to 256, 448] fp16
+ *                      hi/lo coefficient rows (row order permuted for the dedicated kernel when permute != 0; padding rows
+ *                      are not written), xf_d [B, 68] fp32 per-head transform records
+ *   dad3d_flame_decode_from  the product + skinning + projection stage `flags` selects, on caller-written rows and records:
+ *                      the dedicated kernel expects permuted rows (and reads all dec_rows_padded(B) of them), the other paths
+ *                      unpermuted rows.  B must fit one pass of the path (fused_chunk or 4096 heads, see describe), else
+ *                      DAD3D_ERR_INVALID.  The unfused and SIMT paths need dad3d_flame_workspace_bytes(h, B) of workspace
+ *                      (v_posed scratch); the fused paths ignore it
+ *   dad3d_flame_describe  NUL-terminated JSON: basis_scale, jaw_only, nv, npad, fused_chunk, num_sms and, for every pass of a
+ *                      decode of B heads with `flags`, the path ("dedicated", "lbs", "blend", "simt"), rows, m_units (row
+ *                      tiles), splits (vertex-tile ranges per row tile), grid (CTAs of the product kernel), stages and
+ *                      clustered -- computed by the code the launches use */
+DAD3D_API int dad3d_flame_prep(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, void* coef_hi_d, void* coef_lo_d,
+                               float* xf_d, int32_t permute, dad3d_stream stream);
+DAD3D_API int dad3d_flame_decode_from(dad3d_flame* h, const void* coef_hi_d, const void* coef_lo_d, const float* xf_d, int32_t B,
+                                      int32_t flags, float* vertices3d_d, float* projected_d, float image_size, int32_t to_2d,
+                                      void* workspace_d, size_t workspace_bytes, dad3d_stream stream);
+DAD3D_API int dad3d_flame_describe(dad3d_flame* h, int32_t B, int32_t flags, char* json, size_t cap);
+
 /* dad3d_gather_landmarks  replaces np.take(projected_vertices, indices, axis=0) (demo_utils.py:37-47) and
  *   FLAMELayer.indices_2d style subset selection: out[b,l,:] = src[b, idx[l], :].  ncomp = 2 or 3. */
 /* Backward of dad3d_flame_decode (SURVEY §8f row 3): grad_params_d [B, num_params] = d L / d params given
