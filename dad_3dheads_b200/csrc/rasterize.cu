@@ -7,6 +7,9 @@
 //     won by the LOWEST triangle index: one 64-bit atomicMax on (orderable(depth) << 32 | ~index) per covered pixel, then a
 //     per-pixel resolve pass that shades the winner.  alpha must be 1 (what Sim3DR.rasterize passes; blending with alpha < 1 is
 //     order-dependent).
+//   * both passes run over a batch of heads that share one triangle list and colour table (PNCC, depth and triangle-index
+//     maps of a whole predict_batch); each head has its own key words, so a head's result does not depend on the batch.
+//     dad3d_rasterize is the one-head call.
 //   * vertex normals accumulate the un-normalised face normals of the incident triangles in ascending triangle order (caller-built
 //     CSR adjacency), the order of the reference's scatter loop.
 // Integer / float HBM-bound work; no tensor cores.
@@ -59,53 +62,73 @@ __device__ __forceinline__ TriSetup load_tri(const float* __restrict__ v, const 
   return s;
 }
 
-// pass 1: one thread per triangle walks its bounding box
-__global__ void raster_tri_kernel(const float* __restrict__ verts, const int* __restrict__ tris, int ntri, int h, int w,
-                                  const float* __restrict__ depth_in, unsigned long long* __restrict__ key) {
+// pass 1: one thread per (triangle, head) walks the triangle's bounding box.  Heads run along grid y, strided by gridDim.y so
+// that batches past the 65 535 grid-y limit loop; every head offset is 64-bit.
+__global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int batch, const int* __restrict__ tris, int ntri,
+                                  int h, int w, int negate_z, const float* __restrict__ depth_in,
+                                  unsigned long long* __restrict__ key) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= ntri) return;
-  const TriSetup s = load_tri(verts, tris, i);
-  const int x_min = max(static_cast<int>(ceilf(fminf(s.p0x, fminf(s.p1x, s.p2x)))), 0);
-  const int x_max = min(static_cast<int>(floorf(fmaxf(s.p0x, fmaxf(s.p1x, s.p2x)))), w - 1);
-  const int y_min = max(static_cast<int>(ceilf(fminf(s.p0y, fminf(s.p1y, s.p2y)))), 0);
-  const int y_max = min(static_cast<int>(floorf(fmaxf(s.p0y, fmaxf(s.p1y, s.p2y)))), h - 1);
-  if (x_max < x_min || y_max < y_min) return;
-  for (int y = y_min; y <= y_max; ++y)
-    for (int x = x_min; x <= x_max; ++x) {
-      float wt[3];
-      point_weight(wt, static_cast<float>(x), static_cast<float>(y), s.p0x, s.p0y, s.p1x, s.p1y, s.p2x, s.p2y);
-      if (wt[2] > 0 && wt[1] > 0 && wt[0] > 0) {
-        const float d = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
-        if (d > depth_in[y * w + x]) {
-          const unsigned long long k = (static_cast<unsigned long long>(orderable(d)) << 32) |
-                                       static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<unsigned int>(i));
-          atomicMax(&key[y * w + x], k);
+  const long long hw = static_cast<long long>(h) * w;
+  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    TriSetup s = load_tri(verts + static_cast<long long>(b) * nv * 3, tris, i);
+    if (negate_z) { s.d0 = -s.d0; s.d1 = -s.d1; s.d2 = -s.d2; }
+    const int x_min = max(static_cast<int>(ceilf(fminf(s.p0x, fminf(s.p1x, s.p2x)))), 0);
+    const int x_max = min(static_cast<int>(floorf(fmaxf(s.p0x, fmaxf(s.p1x, s.p2x)))), w - 1);
+    const int y_min = max(static_cast<int>(ceilf(fminf(s.p0y, fminf(s.p1y, s.p2y)))), 0);
+    const int y_max = min(static_cast<int>(floorf(fmaxf(s.p0y, fmaxf(s.p1y, s.p2y)))), h - 1);
+    if (x_max < x_min || y_max < y_min) continue;
+    const float* dh = depth_in ? depth_in + b * hw : nullptr;
+    unsigned long long* kh = key + b * hw;
+    for (int y = y_min; y <= y_max; ++y)
+      for (int x = x_min; x <= x_max; ++x) {
+        float wt[3];
+        point_weight(wt, static_cast<float>(x), static_cast<float>(y), s.p0x, s.p0y, s.p1x, s.p1y, s.p2x, s.p2y);
+        if (wt[2] > 0 && wt[1] > 0 && wt[0] > 0) {
+          const float d = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
+          const int pix = y * w + x;
+          if (d > (dh ? dh[pix] : -1e8f)) {                       // Sim3DR.py:22 initialises the buffer to -1e8
+            // d + 0 maps -0 to +0 (and nothing else): the sequential z-test sees -0 and +0 as a tie, the lower index keeps it
+            const unsigned long long k = (static_cast<unsigned long long>(orderable(radd(d, 0.0f))) << 32) |
+                                         static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<unsigned int>(i));
+            atomicMax(&kh[pix], k);
+          }
         }
       }
-    }
+  }
 }
 
-// pass 2: one thread per pixel shades the winning triangle
-__global__ void raster_resolve_kernel(const float* __restrict__ verts, const int* __restrict__ tris, const float* __restrict__ colors,
-                                      int h, int w, int c, int reverse, const unsigned long long* __restrict__ key,
-                                      unsigned char* __restrict__ image, float* __restrict__ depth) {
+// pass 2: one thread per (pixel, head) shades the winning triangle; tri_index gets the winner or -1 in depth-buffer rows
+__global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, int batch, const int* __restrict__ tris,
+                                      const float* __restrict__ colors, int h, int w, int c, int reverse, int negate_z,
+                                      const unsigned long long* __restrict__ key, unsigned char* __restrict__ image,
+                                      float* __restrict__ depth, int* __restrict__ tri_index) {
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= h * w) return;
-  const unsigned long long k = key[pix];
-  if (k == 0ull) return;
-  const int i = static_cast<int>(0xFFFFFFFFu - static_cast<unsigned int>(k & 0xFFFFFFFFull));
+  const long long hw = static_cast<long long>(h) * w;
+  if (pix >= hw) return;
   const int y = pix / w, x = pix - y * w;
-  const TriSetup s = load_tri(verts, tris, i);
-  float wt[3];
-  point_weight(wt, static_cast<float>(x), static_cast<float>(y), s.p0x, s.p0y, s.p1x, s.p1y, s.p2x, s.p2y);
-  depth[pix] = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
   const int yo = reverse ? (h - 1 - y) : y;
-  for (int ch = 0; ch < c; ++ch) {
-    const float pc = radd(radd(rmul(wt[0], colors[c * s.i0 + ch]), rmul(wt[1], colors[c * s.i1 + ch])), rmul(wt[2], colors[c * s.i2 + ch]));
-    // (unsigned char)((1 - alpha) * image + alpha * 255 * p_color) with alpha = 1
-    const float old = static_cast<float>(image[(yo * w + x) * c + ch]);
-    const float val = radd(rmul(rsub(1.0f, 1.0f), old), rmul(rmul(1.0f, 255.0f), pc));
-    image[(yo * w + x) * c + ch] = static_cast<unsigned char>(static_cast<int>(val));
+  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    const long long at = b * hw + pix;
+    const unsigned long long k = key[at];
+    const int i = k == 0ull ? -1 : static_cast<int>(0xFFFFFFFFu - static_cast<unsigned int>(k & 0xFFFFFFFFull));
+    if (tri_index) tri_index[at] = i;
+    if (i < 0) continue;
+    const float* vh = verts + static_cast<long long>(b) * nv * 3;
+    TriSetup s = load_tri(vh, tris, i);
+    if (negate_z) { s.d0 = -s.d0; s.d1 = -s.d1; s.d2 = -s.d2; }
+    float wt[3];
+    point_weight(wt, static_cast<float>(x), static_cast<float>(y), s.p0x, s.p0y, s.p1x, s.p1y, s.p2x, s.p2y);
+    if (depth) depth[at] = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
+    if (!image) continue;
+    unsigned char* px = image + (b * hw + static_cast<long long>(yo) * w + x) * c;
+    for (int ch = 0; ch < c; ++ch) {
+      const float pc = radd(radd(rmul(wt[0], colors[c * s.i0 + ch]), rmul(wt[1], colors[c * s.i1 + ch])), rmul(wt[2], colors[c * s.i2 + ch]));
+      // (unsigned char)((1 - alpha) * image + alpha * 255 * p_color) with alpha = 1
+      const float old = static_cast<float>(px[ch]);
+      const float val = radd(rmul(rsub(1.0f, 1.0f), old), rmul(rmul(1.0f, 255.0f), pc));
+      px[ch] = static_cast<unsigned char>(static_cast<int>(val));
+    }
   }
 }
 
@@ -137,22 +160,41 @@ using namespace dad3d;
 
 extern "C" {
 
-int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri, uint8_t* image_d,
-                    float* depth_d, unsigned long long* key_ws_d, int32_t h, int32_t w, int32_t c, int32_t reverse,
-                    dad3d_stream stream_) {
-  DAD3D_REQUIRE(vertices_d && triangles_d && colors_d && image_d && depth_d && key_ws_d, "null pointer");
-  DAD3D_REQUIRE(ntri >= 0 && h > 0 && w > 0 && c > 0 && static_cast<long long>(h) * w < (1ll << 31), "shape");
+int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                          const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
+                          uint8_t* image_d, float* depth_d, int32_t* tri_index_d, unsigned long long* key_ws_d,
+                          dad3d_stream stream_) {
+  DAD3D_REQUIRE(vertices_d && (triangles_d || ntri == 0) && key_ws_d, "null pointer");
+  DAD3D_REQUIRE(!image_d || colors_d, "image_d needs colors_d");
+  DAD3D_REQUIRE(batch >= 0 && nv > 0 && ntri >= 0 && h > 0 && w > 0 && c > 0 && static_cast<long long>(h) * w < (1ll << 31),
+                "shape");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  DAD3D_CUDA_OK(cudaMemsetAsync(key_ws_d, 0, sizeof(unsigned long long) * static_cast<size_t>(h) * w, stream));
-  if (ntri == 0) return DAD3D_OK;
-  raster_tri_kernel<<<(ntri + 127) / 128, 128, 0, stream>>>(vertices_d, triangles_d, ntri, h, w, depth_d, key_ws_d);
+  const size_t hw = static_cast<size_t>(h) * w;
+  if (batch == 0) return DAD3D_OK;
+  if (ntri == 0) {                                   // nothing covers any pixel: image and depth stay, tri_index is all -1
+    if (tri_index_d) DAD3D_CUDA_OK(cudaMemsetAsync(tri_index_d, 0xFF, sizeof(int32_t) * hw * batch, stream));
+    return DAD3D_OK;
+  }
+  DAD3D_CUDA_OK(cudaMemsetAsync(key_ws_d, 0, sizeof(unsigned long long) * hw * batch, stream));
+  const unsigned int gy = static_cast<unsigned int>(batch < 65535 ? batch : 65535);
+  raster_tri_kernel<<<dim3((ntri + 127) / 128, gy), 128, 0, stream>>>(vertices_d, nv, batch, triangles_d, ntri, h, w,
+                                                                       negate_z, depth_d, key_ws_d);
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
-  raster_resolve_kernel<<<(h * w + 255) / 256, 256, 0, stream>>>(vertices_d, triangles_d, colors_d, h, w, c, reverse, key_ws_d,
-                                                                 image_d, depth_d);
+  raster_resolve_kernel<<<dim3(static_cast<unsigned int>((hw + 255) / 256), gy), 256, 0, stream>>>(
+      vertices_d, nv, batch, triangles_d, colors_d, h, w, c, reverse, negate_z, key_ws_d, image_d, depth_d, tri_index_d);
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
+}
+
+int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri, uint8_t* image_d,
+                    float* depth_d, unsigned long long* key_ws_d, int32_t h, int32_t w, int32_t c, int32_t reverse,
+                    dad3d_stream stream) {
+  DAD3D_REQUIRE(vertices_d && triangles_d && colors_d && image_d && depth_d && key_ws_d, "null pointer");
+  // nv only sets the stride between heads, which one head never uses: 1 stands in for the vertex count this call lacks
+  return dad3d_rasterize_batch(vertices_d, 1, 1, triangles_d, ntri, colors_d, c, h, w, reverse, 0, image_d, depth_d, nullptr,
+                               key_ws_d, stream);
 }
 
 int dad3d_vertex_normals(const float* vertices_d, const int32_t* triangles_d, const int32_t* adj_offsets_d,

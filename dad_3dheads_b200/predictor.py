@@ -5,7 +5,8 @@
 stages and their helper names, so ``demo.py`` / ``demo_utils.py`` code written against the reference keeps working.
 What changes is where the arithmetic runs: ``self.model`` is the CUDA encoder (csrc/encoder.cu) instead of a TorchScript
 module, and ``self.head_mesh`` decodes on the GPU (csrc/flame.cu), once instead of twice per image.
-``predict_batch`` is the batched, device-resident entry point the reference does not have (SURVEY §8b).
+``predict_batch`` is the batched, device-resident entry point the reference does not have (SURVEY §8b); with ``render`` it
+also draws the PNCC, depth and triangle-index maps of every head (rasterizer.PnccRenderer) inside the same step.
 """
 from __future__ import annotations
 
@@ -22,11 +23,13 @@ from . import _lib
 from .encoder import OUTPUT_2D_LANDMARKS, OUTPUT_3DMM_PARAMS, OUTPUT_LANDMARKS_HEATMAP, Dad3dEncoder
 from .flame import load_flame_static
 from .head_mesh import HeadMesh
+from .rasterizer import PnccRenderer
 
 logger = logging.getLogger(__name__)
 _FILENAME = "dad_3dheads.trcd"
 _MEAN = (0.485, 0.456, 0.406)
 _STD = (0.229, 0.224, 0.225)
+RENDER_KEYS = ("pncc", "depth", "tri_index")
 
 DEFAULT_CONFIG = {                                   # == the reference's dad_3dnet.yaml
     "model_path": ".dad_checkpoints/dad_3dheads.trcd",
@@ -105,6 +108,7 @@ class FaceMeshPredictor:
         self._static = None
         self._lm_index: Dict[str, Tensor] = {}
         self._graphs: Dict[Any, Any] = {}
+        self._renderer: Optional[PnccRenderer] = None
 
     # ------------------------------------------------------------------ reference single-image API
     def __call__(self, x: Any) -> Any:
@@ -250,13 +254,33 @@ class FaceMeshPredictor:
             self._lm_index[subset] = torch.from_numpy(self._static[key].astype(np.int64)).to(self.device)
         return self._lm_index[subset]
 
+    @staticmethod
+    def _render_keys(render, to_2d: bool) -> Tuple[str, ...]:
+        """``render`` as a canonical tuple (the order of RENDER_KEYS), validated."""
+        if render is None:
+            return ()
+        if isinstance(render, str):
+            render = (render,)
+        unknown = set(render) - set(RENDER_KEYS)
+        if unknown:
+            raise ValueError(f"render: unknown maps {sorted(unknown)}; choose from {RENDER_KEYS}")
+        keys = tuple(k for k in RENDER_KEYS if k in render)
+        if keys and to_2d:
+            raise ValueError("render needs to_2d=False: the renderer takes the projected vertices with their depth")
+        return keys
+
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
-                      fast_decode: bool = True) -> Dict[str, Tensor]:
+                      fast_decode: bool = True, render=None) -> Dict[str, Tensor]:
         """images: [B,3,256,256] fp32 already letter-boxed + normalised, or raw RGB as the reference's ``__call__`` takes it:
         one [B,H,W,3] uint8 tensor / a list of HxWx3 uint8 images (letter-boxed + normalised on the GPU, bit-identical to
         the reference's albumentations pipeline); host or device.  All outputs stay on the GPU:
         "3dmm_params" [B,413], "points" [B,68,2] (pixels of the 256x256 network input), "3d_vertices" [B,5023,3],
-        "projected_vertices" [B,5023,2|3], "landmarks_<subset>" [B,L,2|3]."""
+        "projected_vertices" [B,5023,2|3], "landmarks_<subset>" [B,L,2|3].
+
+        ``render``: a subset of ("pncc", "depth", "tri_index") (needs ``to_2d=False``) adds those maps of every head, drawn
+        by :class:`~dad_3dheads_b200.rasterizer.PnccRenderer` from "projected_vertices" at the network input size, in the
+        frame of "points": "pncc" [B,S,S,3] uint8, "depth" [B,S,S] fp32, "tri_index" [B,S,S] int32."""
+        render = self._render_keys(render, to_2d)
         if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
             x = self.preprocess_batch(images)
         else:
@@ -268,6 +292,11 @@ class FaceMeshPredictor:
         if landmark_subset is not None:
             dec = self.head_mesh.flame.decoder(self.device)
             out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
+        if render:
+            if self._renderer is None:                       # uploads its tables once (graph-capture safe afterwards)
+                self._renderer = PnccRenderer(self.device)
+            out.update(self._renderer(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
+                                      tri_index="tri_index" in render))
         return out
 
     def _ws_generation(self):
@@ -275,22 +304,22 @@ class FaceMeshPredictor:
         dec = self.head_mesh.flame.decoder(self.device)
         return (self.model.ws_generation, dec.ws_generation)
 
-    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode):
+    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None):
         """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph."""
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             for _ in range(2):
-                self.predict_batch(static_in, landmark_subset, to_2d, fast_decode)
+                self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            out = self.predict_batch(static_in, landmark_subset, to_2d, fast_decode)
+            out = self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render)
         return graph, out, self._ws_generation()
 
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
-                              fast_decode: bool = True) -> Dict[str, Tensor]:
+                              fast_decode: bool = True, render=None) -> Dict[str, Tensor]:
         """:meth:`predict_batch` replayed from a CUDA graph (one graph per input shape / dtype / option set): the ~110 kernel
         launches of a step become one graph launch, which removes the launch gaps between the many sub-20 us layers.
         ``images`` is copied into the graph's static input buffer (host or device source); the returned tensors are the
@@ -300,7 +329,8 @@ class FaceMeshPredictor:
         later call (a larger batch, eager or graphed) reallocates one, every graph captured against the old buffer is
         re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
-        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode)
+        render = self._render_keys(render, to_2d)
+        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render)
         ent = self._graphs.get(key)
         if ent is not None and ent[3] != self._ws_generation():
             ent = None                                        # scratch moved since the capture: never replay it
@@ -308,7 +338,7 @@ class FaceMeshPredictor:
         if ent is None:
             static_in = torch.empty(images.shape, dtype=images.dtype, device=self.device)
             static_in.copy_(images, non_blocking=True)
-            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode)
+            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render)
             ent = (graph, static_in, out, gen)
             self._graphs[key] = ent
         graph, static_in, out, _ = ent
@@ -329,11 +359,12 @@ class BatchStream:
     the requested outputs into pinned host buffers on a fourth stream.  ``collect()`` blocks until the OLDEST submitted batch
     has landed and returns its results.  With ``depth`` slots (default 2) the copies and the collective of batch i overlap
     the encoder of batch i+1, so steady-state throughput is the compute time alone.  Results stay valid until ``depth`` more
-    batches have been submitted.
+    batches have been submitted.  ``render`` is passed to ``predict_batch`` (with ``to_2d=False``); list the maps in
+    ``keys`` to have them copied to the host like the other outputs.
     """
 
     def __init__(self, predictor: FaceMeshPredictor, shape, dtype=torch.uint8, landmark_subset: Optional[str] = "445",
-                 to_2d: bool = True, fast_decode: bool = True, depth: int = 2,
+                 to_2d: bool = True, fast_decode: bool = True, depth: int = 2, render=None,
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
                  group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None):
         self.pred = predictor
@@ -349,7 +380,7 @@ class BatchStream:
         self.copy_in = torch.cuda.Stream(dev)
         self.copy_out = torch.cuda.Stream(dev)
         self.comm = torch.cuda.Stream(dev) if group is not None else None
-        self._args = (landmark_subset, to_2d, fast_decode)
+        self._args = (landmark_subset, to_2d, fast_decode, predictor._render_keys(render, to_2d))
         self.slots = []
         with torch.cuda.device(dev):
             for _ in range(self.depth):

@@ -1,9 +1,14 @@
 """GPU drop-in for the reference's ``Sim3DR`` package (Sim3DR/Sim3DR.py:8-29): ``rasterize`` and ``get_normal`` with the same
 signatures, numpy in / numpy out, bit-exact with the C++ rasteriser they wrap (csrc/rasterize.cu, SURVEY §8f row 4).  Used by
-the reference's ``inference/pncc_estimator.py`` through ``compat/Sim3DR``.  No CPU fallback."""
+the reference's ``inference/pncc_estimator.py`` through ``compat/Sim3DR``.  No CPU fallback.
+
+``rasterize_batch`` and ``PnccRenderer`` are the batched, device-resident form: B heads of one topology per call, device
+tensors in and out, no host synchronisation (so they run inside a captured CUDA graph); every head equals, bit for bit, what
+``rasterize`` gives for that head alone."""
 from __future__ import annotations
 
-from typing import Optional
+import os
+from typing import Dict, Optional
 
 import numpy as np
 import torch
@@ -74,3 +79,117 @@ def get_normal(vertices: np.ndarray, triangles: np.ndarray, cuda_id: Optional[in
         _lib.check(lib.dad3d_vertex_normals(v.data_ptr(), t.data_ptr(), o.data_ptr(), a.data_ptr(), nver, out.data_ptr(),
                                             torch.cuda.current_stream(dev).cuda_stream), "dad3d_vertex_normals")
         return out.cpu().numpy()
+
+
+def _check_triangles(triangles: torch.Tensor, nv: int) -> None:
+    """Bounds-check the triangle indices against ``nv`` on the host, once per tensor and content version: the kernels index
+    vertices through them unchecked.  The first call on a tensor reads it back (a synchronisation); later calls, e.g. inside
+    a graph capture after the warm-up, do not."""
+    tag = (nv, triangles._version)
+    if getattr(triangles, "_dad3d_checked", None) == tag:
+        return
+    if triangles.numel():
+        lo, hi = (int(x) for x in torch.aminmax(triangles))
+        if lo < 0 or hi >= nv:
+            raise ValueError(f"triangle indices span [{lo}, {hi}], outside the {nv} vertices")
+    triangles._dad3d_checked = tag
+
+
+def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Optional[torch.Tensor] = None, *, height: int,
+                    width: int, image: Optional[torch.Tensor] = None, depth: bool = True, tri_index: bool = True,
+                    reverse: bool = False, negate_z: bool = False) -> Dict[str, torch.Tensor]:
+    """Z-buffer rendering of B heads that share one mesh topology, on the GPU (``dad3d_rasterize_batch``).
+
+    vertices [B,nv,3] float32 (x, y in pixels, z = depth, larger wins; with ``negate_z`` -z is the depth), triangles [ntri,3]
+    int32, colors [nv,C] float32 in [0,1] or None (no image), all on one CUDA device.  Returns a dict of the requested maps:
+    "image" [B,height,width,C] uint8 (when ``colors`` is given: zeros, or a copy of ``image``, with the heads drawn over it;
+    ``reverse`` flips its rows), "depth" [B,height,width] float32 (-1e8 where no triangle covers the pixel), "tri_index"
+    [B,height,width] int32 (the winning triangle, -1 for background, in depth-map rows).  Runs on the current stream without
+    a host synchronisation, except the first bounds check of a ``triangles`` tensor."""
+    if vertices.ndim != 3 or vertices.shape[2] != 3 or vertices.dtype != torch.float32 or not vertices.is_cuda:
+        raise ValueError("vertices must be a [B,nv,3] float32 CUDA tensor")
+    if triangles.ndim != 2 or triangles.shape[1] != 3 or triangles.dtype != torch.int32 or triangles.device != vertices.device:
+        raise ValueError("triangles must be an [ntri,3] int32 tensor on the vertices' device")
+    dev = vertices.device
+    B, nv = int(vertices.shape[0]), int(vertices.shape[1])
+    height, width = int(height), int(width)
+    if nv == 0 or height <= 0 or width <= 0 or height * width >= 1 << 31:
+        raise ValueError(f"bad shape: nv={nv}, height={height}, width={width}")
+    vertices = vertices.contiguous()
+    triangles = triangles.contiguous()
+    _check_triangles(triangles, nv)
+    out: Dict[str, torch.Tensor] = {}
+    c = 1
+    if colors is not None:
+        if colors.ndim != 2 or colors.shape[0] != nv or colors.dtype != torch.float32 or colors.device != dev:
+            raise ValueError("colors must be an [nv,C] float32 tensor on the vertices' device")
+        colors = colors.contiguous()
+        c = int(colors.shape[1])
+        if image is None:
+            out["image"] = torch.zeros(B, height, width, c, dtype=torch.uint8, device=dev)
+        else:
+            if tuple(image.shape) != (B, height, width, c) or image.dtype != torch.uint8:
+                raise ValueError(f"image must be [{B},{height},{width},{c}] uint8")
+            out["image"] = image.to(dev, copy=True).contiguous()
+    elif image is not None:
+        raise ValueError("image needs colors")
+    if depth:
+        out["depth"] = torch.full((B, height, width), -1e8, dtype=torch.float32, device=dev)     # Sim3DR.py:22
+    if tri_index:
+        out["tri_index"] = torch.empty(B, height, width, dtype=torch.int32, device=dev)
+    key = torch.empty(B * height * width, dtype=torch.int64, device=dev)       # caching allocator: capture-safe
+    ptr = lambda name: out[name].data_ptr() if name in out else None           # noqa: E731
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        _lib.check(lib.dad3d_rasterize_batch(vertices.data_ptr(), nv, B, triangles.data_ptr(), int(triangles.shape[0]),
+                                             colors.data_ptr() if colors is not None else None, c, height, width,
+                                             1 if reverse else 0, 1 if negate_z else 0, ptr("image"), ptr("depth"),
+                                             ptr("tri_index"), key.data_ptr(), torch.cuda.current_stream(dev).cuda_stream),
+                   "dad3d_rasterize_batch")
+    return out
+
+
+_RENDER_ASSET = os.path.join(os.path.dirname(os.path.abspath(__file__)), "assets", "render_static.json")
+
+
+def load_render_static() -> Dict[str, np.ndarray]:
+    """The reference's PNCC inputs (inference/pncc_estimator.py:66-68), packed by tools/pack_flame_assets.py:
+    "faces_wo_ears" [6270,3] int32, FLAME's faces without the ears (stored as row ranges of the packed FLAME faces), and
+    "ncc_colors" [5023,3] float32, the NCC colour of every template vertex."""
+    import json
+    from .flame import load_flame_static
+    with open(_RENDER_ASSET) as f:
+        d = json.load(f)
+    faces = load_flame_static()["faces"]
+    rows = np.concatenate([np.arange(a, b) for a, b in d["face_rows"]])
+    return {"faces_wo_ears": np.ascontiguousarray(faces[rows], dtype=np.int32),
+            "ncc_colors": np.asarray(d["ncc_colors"], dtype=np.float32)}
+
+
+class PnccRenderer:
+    """The reference's PNCC render (inference/pncc_estimator.py:16-43,66-93) for a batch of decoded heads: the FLAME
+    template's normalised coordinates as colours over the faces without ears, z negated, on a black background.
+
+    ``__call__(projected_vertices_3d, size)`` takes [B,5023,3] float32 on the device, as ``HeadMesh.decode(...,
+    to_2d=False)`` / ``reprojected_vertices(..., to_2d=False)`` return it, and returns {"pncc": [B,S,S,3] uint8, "depth":
+    [B,S,S] float32 (-z; -1e8 for background), "tri_index": [B,S,S] int32 (index into ``faces``, -1 for background)}.
+    ``faces`` and ``colors`` (:func:`load_render_static`) are uploaded once."""
+
+    def __init__(self, device=None):
+        if not torch.cuda.is_available():
+            raise _lib.Dad3dError("PnccRenderer needs a CUDA (sm_90a) device: there is no CPU path")
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        st = load_render_static()
+        self.faces = torch.from_numpy(st["faces_wo_ears"]).to(self.device)
+        self.colors = torch.from_numpy(st["ncc_colors"]).to(self.device)
+        _check_triangles(self.faces, int(self.colors.shape[0]))
+
+    def __call__(self, projected_vertices_3d: torch.Tensor, size: int, *, pncc: bool = True, depth: bool = True,
+                 tri_index: bool = True) -> Dict[str, torch.Tensor]:
+        if projected_vertices_3d.ndim != 3 or projected_vertices_3d.shape[1:] != (self.colors.shape[0], 3):
+            raise ValueError(f"expected [B,{self.colors.shape[0]},3] vertices, got {tuple(projected_vertices_3d.shape)}")
+        out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=size, width=size,
+                              depth=depth, tri_index=tri_index, negate_z=True)
+        if pncc:
+            out["pncc"] = out.pop("image")
+        return out

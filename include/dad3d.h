@@ -265,11 +265,25 @@ DAD3D_API int dad3d_allgather_outputs(dad3d_comm* c, const void* send_d, void* r
  *     (x, y in pixels, z = depth, larger wins), triangles_d [ntri,3], colors_d [nv,c] in [0,1]; image_d [h,w,c] uint8 and
  *     depth_d [h,w] are read-modify-write exactly like the reference's buffers (depth is usually initialised to -1e8);
  *     key_ws_d = h*w 64-bit words of scratch; reverse != 0 flips the image rows.
+ *   dad3d_rasterize_batch: the same for `batch` heads of one topology in two launches, replacing a Python loop of
+ *     Sim3DR.rasterize calls (Sim3DR/Sim3DR.py:13-29; inference/pncc_estimator.py:16-43,66-68,76-93 per head).
+ *     vertices_d [batch,nv,3]; triangles_d [ntri,3] and colors_d [nv,c] are shared by every head.  Outputs, each may be NULL:
+ *     image_d [batch,h,w,c] uint8 and depth_d [batch,h,w] fp32 are read-modify-write exactly as in dad3d_rasterize (with
+ *     depth_d NULL the z-test threshold is the constant -1e8 of Sim3DR.py:22); tri_index_d [batch,h,w] int32 is written for
+ *     every pixel with the winning triangle or -1, in depth-buffer rows (reverse flips only the image).  negate_z != 0 uses -z
+ *     as depth (pncc_estimator.py:77 `vertices[:, :, 2] *= -1`; exact, since negation commutes with rounding).  colors_d may
+ *     be NULL when image_d is, triangles_d when ntri = 0.  key_ws_d = batch*h*w 64-bit words of scratch.  Every head equals, bit for bit, a
+ *     single-head call on that head.  batch = 0 launches nothing; ntri = 0 launches nothing and sets tri_index_d to -1.
+ *     dad3d_rasterize is the batch = 1 call of these kernels.
  *   dad3d_vertex_normals: normalised sum of the incident (un-normalised) face normals per vertex; adj_offsets_d [nv+1] /
  *     adj_triangles_d = CSR list of each vertex's triangles in ascending order (fixed per topology). */
 DAD3D_API int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri,
                               uint8_t* image_d, float* depth_d, unsigned long long* key_ws_d, int32_t h, int32_t w, int32_t c,
                               int32_t reverse, dad3d_stream stream);
+DAD3D_API int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                                    const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
+                                    uint8_t* image_d, float* depth_d, int32_t* tri_index_d, unsigned long long* key_ws_d,
+                                    dad3d_stream stream);
 DAD3D_API int dad3d_vertex_normals(const float* vertices_d, const int32_t* triangles_d, const int32_t* adj_offsets_d,
                                    const int32_t* adj_triangles_d, int32_t nver, float* normals_d, dad3d_stream stream);
 

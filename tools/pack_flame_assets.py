@@ -11,6 +11,14 @@ What is read (reference data assets, not source):
   model_training/model/static/face_keypoints/keypoints_{191,445}/*.npy   (demo_utils.py:37-47, model_training/utils.py:81-105)
   model_training/model/static/flame_static_embedding.pkl, flame_dynamic_embedding.npy (data/utils.py:120-206)
 
+and, into a second small text file ``render_static.json`` (read by ``rasterizer.load_render_static``), the two inputs of the
+reference's PNCC renderer (inference/pncc_estimator.py:46-60,66-68):
+  model_training/model/static/flame_indices/faces_wo_ears_remapped.npy  -> ``face_rows``: that file is FLAME's face list
+  with the ear faces removed, in order, so it is stored as [start, stop) row ranges of ``faces`` in flame_static.npz
+  ``ncc_colors`` [5023,3]: the template normalised to the unit cube over the vertices those faces use, computed in fp64 from
+  the fp64 template of flame.pkl and rounded to fp32 once (as Sim3DR.rasterize does); from the packed fp32 template the
+  last bits would differ.  Written as the shortest decimals that read back to the same fp32 values.
+
 The pickle is python-2 era and references ``chumpy.ch.Ch`` + ``scipy.sparse.csc.csc_matrix``; chumpy is not installed, so
 a restricted unpickler substitutes a stub for it (its array payload is attribute ``x``).
 """
@@ -86,13 +94,57 @@ def _keypoint_subset(dirpath, exclude=()):
     return np.asarray(idx, dtype=np.int32), per_file
 
 
+def ncc_color_codes(template: np.ndarray, faces: np.ndarray) -> np.ndarray:
+    """(template - lo) / (hi - lo) per axis, lo / hi the extent of the vertices ``faces`` uses with 0 included (the
+    ``initial=0`` of pncc_estimator.py:53-54), in the template's own precision."""
+    sub = template[np.unique(faces)]
+    lo = sub.min(axis=0, keepdims=True, initial=0)
+    hi = sub.max(axis=0, keepdims=True, initial=0)
+    return (template - lo) / (hi - lo)
+
+
+def face_row_ranges(faces: np.ndarray, subset: np.ndarray) -> list:
+    """[start, stop) row ranges of ``faces`` whose concatenation is ``subset`` (which must be an ordered subset of rows)."""
+    rows = {tuple(r): i for i, r in enumerate(faces.tolist())}
+    idx = np.array([rows[tuple(r)] for r in subset.tolist()])
+    if not np.all(np.diff(idx) > 0):
+        raise ValueError("subset is not an ordered subset of the face rows")
+    cut = np.flatnonzero(np.diff(idx) != 1) + 1
+    return [[int(r[0]), int(r[-1]) + 1] for r in np.split(idx, cut)]
+
+
+def pack_render_static(st: str, out_path: str) -> None:
+    import json
+    fl = _load_pickle(os.path.join(st, "flame.pkl"))
+    template = _np(fl["v_template"], np.float64)
+    flame_faces = _np(fl["f"]).astype(np.int32)
+    faces = np.load(os.path.join(st, "flame_indices", "faces_wo_ears_remapped.npy")).astype(np.int32)
+    ranges = face_row_ranges(flame_faces, faces)
+    colors = ncc_color_codes(template, faces).astype(np.float32)
+    dec = [[np.format_float_positional(x, unique=True, trim="-") for x in row] for row in colors]
+    back = np.array([[float(x) for x in row] for row in dec], np.float32)
+    assert np.array_equal(back.view(np.uint32), colors.view(np.uint32)), "decimal round trip"
+    with open(out_path, "w") as f:
+        f.write('{"face_rows": ' + json.dumps(ranges, separators=(",", ":")) + ',\n "ncc_colors": [\n')
+        f.write(",\n".join("[" + ",".join(row) + "]" for row in dec))
+        f.write("]}\n")
+    print("wrote", os.path.abspath(out_path), os.path.getsize(out_path) / 1e3, "kB")
+
+
 def main():
+    assets = os.path.join(os.path.dirname(__file__), "..", "dad_3dheads_b200", "assets")
     ap = argparse.ArgumentParser()
     ap.add_argument("--ref", default=REF)
-    ap.add_argument("--out", default=os.path.join(os.path.dirname(__file__), "..", "dad_3dheads_b200", "assets",
-                                                  "flame_static.npz"))
+    ap.add_argument("--out", default=os.path.join(assets, "flame_static.npz"))
+    ap.add_argument("--render-out", default=os.path.join(assets, "render_static.json"))
+    ap.add_argument("--only", choices=("flame_static", "render_static"), default=None,
+                    help="write one of the two files (default: both)")
     args = ap.parse_args()
     st = os.path.join(args.ref, STATIC)
+    if args.only != "flame_static":
+        pack_render_static(st, args.render_out)
+    if args.only == "render_static":
+        return
 
     fl = _load_pickle(os.path.join(st, "flame.pkl"))
     v_template = _np(fl["v_template"], np.float32)                      # [5023,3]
