@@ -65,6 +65,12 @@ SIGNATURES = {
                                    C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_preprocess_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_roi_setup": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "dad3d_preprocess_rois": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_readjust_rois": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_rasterize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "dad3d_rasterize_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,

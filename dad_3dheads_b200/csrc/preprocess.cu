@@ -1,72 +1,29 @@
-// Device-side image pre-processing (SURVEY §8f "next" row 2): the reference's albumentations pipeline
-//   LongestMaxSize(256, cv2.INTER_LINEAR on uint8) -> PadIfNeeded(256, 256, constant 0, centred) -> Normalize(imagenet)
-//   -> HWC->CHW   (predictor.py:195-203, :85-89)
-// in one kernel per image: uint8 RGB [H,W,3] (device) -> fp32 [3,S,S] slot of the encoder's input batch.
-// The bilinear resize restates OpenCV's 8-bit fixed-point path bit-exactly (11-bit coefficients, horizontal taps clamped
-// with zeroed fraction, vertical taps clamped by row index only, two-step rounded vertical blend); the normalisation
-// uses the same two fp32 roundings as albumentations (subtract mean*255, multiply by 1/(std*255)).
+// Device-side image pre-processing (SURVEY §8f "next" row 2): the letter-box of letterbox.cuh in one kernel per image batch:
+// uint8 RGB [H,W,3] (device) -> fp32 [3,S,S] slot of the encoder's input batch.
 #include <cstdint>
 
 #include "../../include/dad3d.h"
 #include "common.h"
+#include "letterbox.cuh"
 
 namespace dad3d {
 
 struct PreParams {
-  int H, W, nh, nw, top, left, S, do_resize;
-  double scale_x, scale_y;
+  LetterboxGeom g;
+  int S;
   float mean[3], inv_std[3];
 };
-
-__device__ __forceinline__ void lin_coeff(int d, double scale, int n_src, bool clamp_frac, int* s0, int* s1, int* a0, int* a1) {
-  float f = static_cast<float>((static_cast<double>(d) + 0.5) * scale - 0.5);
-  int s = static_cast<int>(floorf(f));
-  f -= static_cast<float>(s);
-  if (clamp_frac) {                         // cv::resize horizontal pass: out-of-range taps collapse onto the border pixel
-    if (s < 0) { f = 0.f; s = 0; }
-    if (s >= n_src - 1) { f = 0.f; s = n_src - 1; }
-  }
-  int c0 = __float2int_rn((1.f - f) * 2048.f);     // saturate_cast<short>(float): round half to even
-  int c1 = __float2int_rn(f * 2048.f);
-  c0 = max(-32768, min(32767, c0));
-  c1 = max(-32768, min(32767, c1));
-  *a0 = c0;
-  *a1 = c1;
-  *s0 = max(0, min(n_src - 1, s));                  // vertical pass: rows are clamped, the fraction is kept
-  *s1 = max(0, min(n_src - 1, s + 1));
-}
 
 // blockIdx.z = image of a same-sized batch ([B,H,W,3] uint8 -> [B,3,S,S] fp32); a single image is the B = 1 case
 __global__ void preprocess_kernel(const uint8_t* __restrict__ img, PreParams p, float* __restrict__ out) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   const int y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= p.S || y >= p.S) return;
-  img += static_cast<size_t>(blockIdx.z) * p.H * p.W * 3;
+  img += static_cast<size_t>(blockIdx.z) * p.g.H * p.g.W * 3;
   out += static_cast<size_t>(blockIdx.z) * 3 * p.S * p.S;
-  int v[3] = {0, 0, 0};
-  const int dx = x - p.left, dy = y - p.top;
-  if (dx >= 0 && dx < p.nw && dy >= 0 && dy < p.nh) {
-    if (!p.do_resize) {
-      const uint8_t* s = img + (static_cast<size_t>(dy) * p.W + dx) * 3;
-      v[0] = s[0]; v[1] = s[1]; v[2] = s[2];
-    } else {
-      int sx0, sx1, ax0, ax1, sy0, sy1, ay0, ay1;
-      lin_coeff(dx, p.scale_x, p.W, true, &sx0, &sx1, &ax0, &ax1);
-      lin_coeff(dy, p.scale_y, p.H, false, &sy0, &sy1, &ay0, &ay1);
-      const uint8_t* r0 = img + static_cast<size_t>(sy0) * p.W * 3;
-      const uint8_t* r1 = img + static_cast<size_t>(sy1) * p.W * 3;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int h0 = r0[sx0 * 3 + c] * ax0 + r0[sx1 * 3 + c] * ax1;
-        const int h1 = r1[sx0 * 3 + c] * ax0 + r1[sx1 * 3 + c] * ax1;
-        const int r = ((((ay0 * (h0 >> 4)) >> 16) + ((ay1 * (h1 >> 4)) >> 16) + 2) >> 2);
-        v[c] = max(0, min(255, r));
-      }
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < 3; ++c)
-    out[(static_cast<size_t>(c) * p.S + y) * p.S + x] = __fmul_rn(__fsub_rn(static_cast<float>(v[c]), p.mean[c]), p.inv_std[c]);
+  int v[3];
+  letterbox_pixel(img, static_cast<size_t>(p.g.W) * 3, p.g, x, y, v);
+  store_normalised(out, p.S, x, y, v, p.mean, p.inv_std);
 }
 
 }  // namespace dad3d
@@ -86,12 +43,12 @@ extern "C" int dad3d_preprocess_batch(const uint8_t* images_d, int32_t B, int32_
   DAD3D_REQUIRE(image_d && out_d && mean255_h && inv_std255_h, "null pointer");
   DAD3D_REQUIRE(H > 0 && W > 0 && new_h > 0 && new_w > 0 && new_h <= img_size && new_w <= img_size, "sizes");
   PreParams p;
-  p.H = H; p.W = W; p.nh = new_h; p.nw = new_w; p.S = img_size;
-  p.top = new_h < img_size ? static_cast<int>((img_size - new_h) / 2.0) : 0;     // PadIfNeeded centring
-  p.left = new_w < img_size ? static_cast<int>((img_size - new_w) / 2.0) : 0;
-  p.do_resize = (new_h != H || new_w != W) ? 1 : 0;
-  p.scale_x = 1.0 / (static_cast<double>(new_w) / W);                             // cv::resize: 1 / inv_scale_x
-  p.scale_y = 1.0 / (static_cast<double>(new_h) / H);
+  p.g.H = H; p.g.W = W; p.g.nh = new_h; p.g.nw = new_w; p.S = img_size;
+  p.g.top = new_h < img_size ? static_cast<int>((img_size - new_h) / 2.0) : 0;     // PadIfNeeded centring
+  p.g.left = new_w < img_size ? static_cast<int>((img_size - new_w) / 2.0) : 0;
+  p.g.do_resize = (new_h != H || new_w != W) ? 1 : 0;
+  p.g.scale_x = 1.0 / (static_cast<double>(new_w) / W);                             // cv::resize: 1 / inv_scale_x
+  p.g.scale_y = 1.0 / (static_cast<double>(new_h) / H);
   for (int c = 0; c < 3; ++c) { p.mean[c] = mean255_h[c]; p.inv_std[c] = inv_std255_h[c]; }
   dim3 block(32, 8), grid(ceil_div(img_size, 32), ceil_div(img_size, 8), B);
   preprocess_kernel<<<grid, block, 0, reinterpret_cast<cudaStream_t>(stream)>>>(image_d, p, out_d);

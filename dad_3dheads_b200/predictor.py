@@ -26,6 +26,8 @@ from .head_mesh import HeadMesh
 from .rasterizer import PnccRenderer
 
 logger = logging.getLogger(__name__)
+ROI_RECORD_BYTES = 72                                # sizeof(dad3d_roi), include/dad3d.h
+MAX_ROIS = 65535                                     # ROIs per call: dad3d_preprocess_rois runs them along grid z
 _FILENAME = "dad_3dheads.trcd"
 _MEAN = (0.485, 0.456, 0.406)
 _STD = (0.229, 0.224, 0.225)
@@ -60,6 +62,18 @@ def calculate_paddings(orig_h: int, orig_w: int) -> List[int]:
     top = int((side - orig_h) / 2)
     left = int((side - orig_w) / 2)
     return [top, side - orig_h - top, left, side - orig_w - left]
+
+
+def extend_sides(extend) -> Tuple[float, float, float, float]:
+    """``extend_bbox``'s offset (model_training/data/utils.py:73-100) -- one fraction, (width, height) or
+    (left, right, top, bottom) -- as the four fractions (left, right, top, bottom)."""
+    if isinstance(extend, (tuple, list)):
+        if len(extend) == 4:
+            return tuple(float(v) for v in extend)
+        if len(extend) == 2:
+            return (float(extend[0]),) * 2 + (float(extend[1]),) * 2
+        raise ValueError(f"extend: a float, a 2-tuple or a 4-tuple, got {len(extend)} values")
+    return (float(extend),) * 4
 
 
 def letterbox_normalise(x: np.ndarray, img_size: int) -> np.ndarray:
@@ -269,8 +283,73 @@ class FaceMeshPredictor:
             raise ValueError("render needs to_2d=False: the renderer takes the projected vertices with their depth")
         return keys
 
+    def _check_rois(self, frames, boxes, frame_index) -> Tuple[Tensor, Optional[Tensor]]:
+        """Validates the frames + boxes arguments before anything is launched -> (boxes, frame_index) as tensors."""
+        if not (isinstance(frames, Tensor) and frames.dtype == torch.uint8 and frames.ndim == 4 and frames.shape[3] == 3):
+            raise ValueError("frames: one [F,H,W,3] uint8 tensor")
+        if min(frames.shape[:3]) < 1:
+            raise ValueError(f"frames: empty shape {tuple(frames.shape)}")
+        ints = (torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64)
+        boxes = torch.as_tensor(boxes)
+        if boxes.dtype not in ints or boxes.ndim != 2 or boxes.shape[1] != 4:
+            raise ValueError(f"boxes: an [R,4] integer tensor of [x, y, w, h], got {boxes.dtype} {tuple(boxes.shape)}")
+        R = int(boxes.shape[0])
+        if R > MAX_ROIS:
+            raise ValueError(f"boxes: at most {MAX_ROIS} per call, got {R}")
+        if frame_index is not None:
+            frame_index = torch.as_tensor(frame_index)
+            if frame_index.dtype not in ints or tuple(frame_index.shape) != (R,):
+                raise ValueError(f"frame_index: an [R] integer tensor, got {frame_index.dtype} {tuple(frame_index.shape)}")
+            F = int(frames.shape[0])
+            if frame_index.device.type == "cpu" and R and (int(frame_index.min()) < 0 or int(frame_index.max()) >= F):
+                raise ValueError(f"frame_index: values must lie in [0, {F})")
+        c = self.flame_constants
+        if c["scale"] != 1 or c["translation"] != 3:
+            raise ValueError("boxes need the released 3DMM layout (one scale, three translation parameters)")
+        return boxes, frame_index
+
+    def _predict_rois(self, frames, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode) -> Dict[str, Tensor]:
+        """predict_batch with boxes: crop geometry, pre-processing and read-back in csrc/roi.cu, no host synchronisation."""
+        boxes, frame_index = self._check_rois(frames, boxes, frame_index)
+        ext = np.array(extend_sides(extend), dtype=np.float64)
+        frames = frames.to(self.device, non_blocking=True).contiguous()
+        boxes = boxes.to(self.device, torch.int32, non_blocking=True).contiguous()
+        if frame_index is not None:
+            frame_index = frame_index.to(self.device, torch.int32, non_blocking=True).contiguous()
+        c = self.flame_constants
+        lib = _lib.load()
+        S = self._img_size
+        F, H, W = (int(d) for d in frames.shape[:3])
+        R = int(boxes.shape[0])
+        mean = (np.array(_MEAN, dtype=np.float32) * 255.0).astype(np.float32)
+        inv = np.reciprocal(np.array(_STD, dtype=np.float32) * 255.0, dtype=np.float32)
+        rois = torch.empty(R, ROI_RECORD_BYTES, dtype=torch.uint8, device=self.device)
+        x = torch.empty(R, 3, S, S, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _lib.check(lib.dad3d_roi_setup(boxes.data_ptr(), frame_index.data_ptr() if frame_index is not None else None, R,
+                                           F, H, W, S, ext.ctypes.data, rois.data_ptr(), stream), "dad3d_roi_setup")
+            _lib.check(lib.dad3d_preprocess_rois(frames.data_ptr(), H, W, rois.data_ptr(), R, S, mean.ctypes.data,
+                                                 inv.ctypes.data, x.data_ptr(), stream), "dad3d_preprocess_rois")
+            raw, lms, _ = self.model.forward_raw(x, want_heatmap=False)
+            params = torch.empty_like(raw)
+            points = torch.empty(R, lms.shape[1], 2, dtype=torch.int64, device=self.device)
+            _lib.check(lib.dad3d_readjust_rois(raw.data_ptr(), lms.data_ptr(), rois.data_ptr(), R, raw.shape[1],
+                                               lms.shape[1], self.find_3dmm_idx("scale", c),
+                                               self.find_3dmm_idx("translation", c), S, params.data_ptr(),
+                                               points.data_ptr(), stream), "dad3d_readjust_rois")
+        v3, proj = self.head_mesh.decode(params, to_2d=to_2d, hilo=not fast_decode)
+        fields = rois.view(torch.int32)                       # x, y, w, h, frame, valid, ... (dad3d_roi)
+        out = {"3dmm_params": params, "points": points, "3d_vertices": v3, "projected_vertices": proj,
+               "crop_boxes": fields[:, :4].contiguous(), "valid": fields[:, 5] != 0}
+        if landmark_subset is not None:
+            dec = self.head_mesh.flame.decoder(self.device)
+            out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
+        return out
+
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
-                      fast_decode: bool = True, render=None) -> Dict[str, Tensor]:
+                      fast_decode: bool = True, render=None, boxes=None, frame_index=None,
+                      extend=0.0) -> Dict[str, Tensor]:
         """images: [B,3,256,256] fp32 already letter-boxed + normalised, or raw RGB as the reference's ``__call__`` takes it:
         one [B,H,W,3] uint8 tensor / a list of HxWx3 uint8 images (letter-boxed + normalised on the GPU, bit-identical to
         the reference's albumentations pipeline); host or device.  All outputs stay on the GPU:
@@ -279,8 +358,23 @@ class FaceMeshPredictor:
 
         ``render``: a subset of ("pncc", "depth", "tri_index") (needs ``to_2d=False``) adds those maps of every head, drawn
         by :class:`~dad_3dheads_b200.rasterizer.PnccRenderer` from "projected_vertices" at the network input size, in the
-        frame of "points": "pncc" [B,S,S,3] uint8, "depth" [B,S,S] fp32, "tri_index" [B,S,S] int32."""
+        frame of "points": "pncc" [B,S,S,3] uint8, "depth" [B,S,S] fp32, "tri_index" [B,S,S] int32.
+
+        ``boxes``: heads in whole frames.  ``images`` is then one [F,H,W,3] uint8 tensor of frames and ``boxes`` an [R,4]
+        integer tensor of head boxes [x, y, w, h] in frame pixels (host or device), on frame ``frame_index[r]`` ([R]
+        integers; None: every box is on frame 0).  Each box is cropped as the reference's data pipeline does,
+        ``ensure_bbox_boundaries(extend_bbox(box, extend), (H, W))`` (``extend``: a fraction, (width, height) or
+        (left, right, top, bottom)), and each crop gives what ``__call__`` gives on it, moved into frame pixels:
+        "3dmm_params" readjusted to the frame (translation z = 0), "points" [R,68,2] int64 frame pixels, and
+        "projected_vertices" / "landmarks_<subset>" decoded from those parameters; plus "crop_boxes" [R,4] int32 and
+        "valid" [R] bool.  A box is invalid when its frame index is out of range, its crop is empty, or a side of its
+        letter-box rounds to 0 pixels; its outputs are finite but meaningless.  Nothing waits for the device, so boxes
+        computed on the GPU are consumed directly.  At most 65 535 boxes per call; ``render`` is not supported."""
         render = self._render_keys(render, to_2d)
+        if boxes is not None:
+            if render:
+                raise ValueError("render is not supported together with boxes")
+            return self._predict_rois(images, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode)
         if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
             x = self.preprocess_batch(images)
         else:
@@ -304,22 +398,39 @@ class FaceMeshPredictor:
         dec = self.head_mesh.flame.decoder(self.device)
         return (self.model.ws_generation, dec.ws_generation)
 
-    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None):
-        """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph."""
+    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None):
+        """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph.
+        ``rois`` = (static boxes [R,4] int32, static frame index [R] int32, extend): the graph reads the boxes from those
+        buffers on every replay."""
+        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2]) if rois is not None else {}
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
             for _ in range(2):
-                self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render)
+                self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render, **kw)
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            out = self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render)
+            out = self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render, **kw)
         return graph, out, self._ws_generation()
 
+    def _roi_buffers(self, R: int, extend):
+        """Static boxes / frame index buffers of a captured step with R boxes (zero boxes: every ROI invalid until filled)."""
+        return (torch.zeros(R, 4, dtype=torch.int32, device=self.device),
+                torch.zeros(R, dtype=torch.int32, device=self.device), extend_sides(extend))
+
+    @staticmethod
+    def _fill_rois(rois, boxes: Tensor, frame_index: Optional[Tensor]) -> None:
+        rois[0].copy_(boxes, non_blocking=True)
+        if frame_index is None:
+            rois[1].zero_()
+        else:
+            rois[1].copy_(frame_index, non_blocking=True)
+
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
-                              fast_decode: bool = True, render=None) -> Dict[str, Tensor]:
+                              fast_decode: bool = True, render=None, boxes=None, frame_index=None,
+                              extend=0.0) -> Dict[str, Tensor]:
         """:meth:`predict_batch` replayed from a CUDA graph (one graph per input shape / dtype / option set): the ~110 kernel
         launches of a step become one graph launch, which removes the launch gaps between the many sub-20 us layers.
         ``images`` is copied into the graph's static input buffer (host or device source); the returned tensors are the
@@ -327,10 +438,18 @@ class FaceMeshPredictor:
 
         A captured graph holds raw pointers into the encoder / decoder scratch buffers.  Those buffers only ever grow; when a
         later call (a larger batch, eager or graphed) reallocates one, every graph captured against the old buffer is
-        re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced."""
+        re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced.
+
+        With ``boxes`` (see :meth:`predict_batch`) the boxes and frame indices are copied into static buffers as well: one
+        graph serves every box set of the same frame shape, box count and ``extend``."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
         render = self._render_keys(render, to_2d)
         key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render)
+        if boxes is not None:
+            if render:
+                raise ValueError("render is not supported together with boxes")
+            boxes, frame_index = self._check_rois(images, boxes, frame_index)
+            key += (int(boxes.shape[0]), extend_sides(extend))
         ent = self._graphs.get(key)
         if ent is not None and ent[3] != self._ws_generation():
             ent = None                                        # scratch moved since the capture: never replay it
@@ -338,16 +457,22 @@ class FaceMeshPredictor:
         if ent is None:
             static_in = torch.empty(images.shape, dtype=images.dtype, device=self.device)
             static_in.copy_(images, non_blocking=True)
-            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render)
-            ent = (graph, static_in, out, gen)
+            rois = self._roi_buffers(int(boxes.shape[0]), extend) if boxes is not None else None
+            if rois is not None:
+                self._fill_rois(rois, boxes, frame_index)
+            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois)
+            ent = (graph, static_in, out, gen, rois)
             self._graphs[key] = ent
-        graph, static_in, out, _ = ent
+        graph, static_in, out, _, rois = ent
         static_in.copy_(images, non_blocking=True)
+        if rois is not None:
+            self._fill_rois(rois, boxes, frame_index)
         graph.replay()
         return out
 
     def open_stream(self, shape, dtype=torch.uint8, **kw) -> "BatchStream":
-        """A double-buffered pipeline over :meth:`predict_batch` for a fixed batch signature -- see :class:`BatchStream`."""
+        """A double-buffered pipeline over :meth:`predict_batch` for a fixed batch signature -- see :class:`BatchStream`.
+        ``rois=R`` (with optional ``extend``): ``shape`` is that of the frames, and every submit brings R boxes."""
         return BatchStream(self, shape, dtype, **kw)
 
 
@@ -360,13 +485,16 @@ class BatchStream:
     has landed and returns its results.  With ``depth`` slots (default 2) the copies and the collective of batch i overlap
     the encoder of batch i+1, so steady-state throughput is the compute time alone.  Results stay valid until ``depth`` more
     batches have been submitted.  ``render`` is passed to ``predict_batch`` (with ``to_2d=False``); list the maps in
-    ``keys`` to have them copied to the host like the other outputs.
+    ``keys`` to have them copied to the host like the other outputs.  With ``rois=R`` each batch is frames plus R boxes
+    (``predict_batch``'s ``boxes``): ``submit(frames, boxes=, frame_index=)`` copies the boxes on the copy stream together with
+    the frames; "crop_boxes" and "valid" may be listed in ``keys``.
     """
 
     def __init__(self, predictor: FaceMeshPredictor, shape, dtype=torch.uint8, landmark_subset: Optional[str] = "445",
                  to_2d: bool = True, fast_decode: bool = True, depth: int = 2, render=None,
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
-                 group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None):
+                 group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None, rois=None,
+                 extend=0.0):
         self.pred = predictor
         dev = predictor.device
         self.device = dev
@@ -381,12 +509,16 @@ class BatchStream:
         self.copy_out = torch.cuda.Stream(dev)
         self.comm = torch.cuda.Stream(dev) if group is not None else None
         self._args = (landmark_subset, to_2d, fast_decode, predictor._render_keys(render, to_2d))
+        if rois is not None and self._args[3]:
+            raise ValueError("render is not supported together with boxes")
+        self.rois = rois
         self.slots = []
         with torch.cuda.device(dev):
             for _ in range(self.depth):
                 static_in = torch.zeros(tuple(shape), dtype=dtype, device=dev)
-                graph, out, gen = predictor._capture(static_in, *self._args)
-                slot = {"in": static_in, "graph": graph, "out": out, "gen": gen, "busy": False,
+                roi_bufs = predictor._roi_buffers(int(rois), extend) if rois is not None else None
+                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs)
+                slot = {"in": static_in, "rois": roi_bufs, "graph": graph, "out": out, "gen": gen, "busy": False,
                         "h2d": torch.cuda.Event(), "done": torch.cuda.Event(), "comm_done": torch.cuda.Event(),
                         "d2h": torch.cuda.Event(), "gathered": {}, "host": {}}
                 if host_results:
@@ -405,16 +537,24 @@ class BatchStream:
         self._tail = 0          # oldest uncollected
         self._inflight = 0
 
-    def submit(self, images: Tensor) -> None:
+    def submit(self, images: Tensor, boxes=None, frame_index=None) -> None:
         if self._inflight == self.depth:
             raise RuntimeError("BatchStream: all slots in flight -- collect() before submitting more")
+        if (boxes is None) != (self.rois is None):
+            raise ValueError("boxes are required exactly when the stream was opened with rois=")
+        if boxes is not None:
+            boxes, frame_index = self.pred._check_rois(images, boxes, frame_index)
+            if int(boxes.shape[0]) != self.rois:
+                raise ValueError(f"boxes: this stream takes {self.rois} per batch, got {int(boxes.shape[0])}")
         s = self.slots[self._head]
         if s["gen"] != self.pred._ws_generation():           # scratch reallocated by another caller: re-capture this slot
             torch.cuda.synchronize(self.device)
-            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args)
+            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"])
         with torch.cuda.stream(self.copy_in):
             self.copy_in.wait_event(s["done"])               # the previous replay of this slot has consumed its input
             s["in"].copy_(images, non_blocking=True)
+            if boxes is not None:
+                self.pred._fill_rois(s["rois"], boxes, frame_index)
             s["h2d"].record(self.copy_in)
         with torch.cuda.stream(self.compute):
             self.compute.wait_event(s["h2d"])

@@ -78,13 +78,28 @@ class SubmissionWriter:
             rows.append([float(pads[2]), float(pads[0]), scale])
         return torch.tensor(rows, dtype=torch.float32, device=self.pred.device)
 
-    def predict(self, images, item_ids: Iterable[str], input_shapes=None) -> Dict[str, Dict[str, list]]:
+    def predict(self, images, item_ids: Iterable[str], input_shapes=None, boxes=None, frame_index=None,
+                extend=0.0) -> Dict[str, Dict[str, list]]:
         """images: raw RGB frames (list of HxWx3 uint8 arrays/tensors of any sizes, or one [B,H,W,3] uint8 tensor) -- the
         benchmark's inputs -- or an already letter-boxed [B,3,256,256] fp32 batch together with ``input_shapes`` =
         [(h, w), ...] of the originals.  "68_landmarks_2d" is returned in ORIGINAL-image pixels, which is what the evaluator
         compares with its ground truth (dad_3dheads_benchmark/benchmark.py:86-99): the letter-box is undone exactly as
         ``readjust_3dmm_to_the_input_image`` + ``reprojected_vertices`` do in the reference (predictor.py:154-176,
-        head_mesh.py:33-46): xy_orig = (xy_256 - [pad_left, pad_top]) / scale."""
+        head_mesh.py:33-46): xy_orig = (xy_256 - [pad_left, pad_top]) / scale.
+
+        With ``boxes`` ([R,4] integer [x, y, w, h], one per item, as the benchmark's metadata gives them), ``images`` is one
+        [F,H,W,3] uint8 tensor of whole frames and item r is the head in box r on frame ``frame_index[r]`` (default: frame r).
+        The heads are cropped and read back into frame pixels by ``predict_batch(..., boxes=)``, so "68_landmarks_2d" is the
+        barycentric 68 on the frame-space projected vertices: already in the evaluator's full-image frame."""
+        if boxes is not None:
+            R = int(torch.as_tensor(boxes).shape[0])
+            if frame_index is None:
+                if not (isinstance(images, Tensor) and images.ndim == 4 and int(images.shape[0]) == R):
+                    raise ValueError("boxes without frame_index need one frame per box")
+                frame_index = torch.arange(R, dtype=torch.int32)
+            out = self.pred.predict_batch(images, landmark_subset=None, to_2d=True, boxes=boxes, frame_index=frame_index,
+                                          extend=extend)
+            return self._items(self.fields_from_outputs(out), item_ids)
         if input_shapes is None:
             if isinstance(images, (list, tuple)):
                 input_shapes = [tuple(int(d) for d in torch.as_tensor(im).shape[:2]) for im in images]
@@ -95,6 +110,10 @@ class SubmissionWriter:
         if input_shapes is not None:
             geo = self.letterbox_geometry(input_shapes)                            # [B,3]
             fields["68_landmarks_2d"] = (fields["68_landmarks_2d"] - geo[:, None, :2]) / geo[:, None, 2:3]
+        return self._items(fields, item_ids)
+
+    @staticmethod
+    def _items(fields: Dict[str, Tensor], item_ids: Iterable[str]) -> Dict[str, Dict[str, list]]:
         f = {k: v.detach().cpu() for k, v in fields.items()}
         res = {}
         for i, item in enumerate(item_ids):

@@ -188,6 +188,45 @@ DAD3D_API int dad3d_preprocess_batch(const uint8_t* images_d, int32_t B, int32_t
                                      int32_t img_size, const float* mean255_h, const float* inv_std255_h, float* out_d,
                                      dad3d_stream stream);
 
+/* ---- heads from boxes in whole frames ----------------------------------------------------------------------------------
+ * What a caller of the reference does per head box: crop (model_training/data/flame_dataset.py:96-99), run
+ * FaceMeshPredictor.__call__ on the crop (predictor.py:117-176) and move the result into frame pixels -- for R boxes at once,
+ * with every geometric value computed on the device, so the boxes may change between replays of a captured graph.
+ *   dad3d_roi_setup  boxes_d [R,4] int32 [x, y, w, h] in frame pixels, frame_index_d [R] int32 (NULL: every box is on frame 0)
+ *     -> rois_d [R] records.  crop = ensure_bbox_boundaries(extend_bbox(box, extend), (H, W)) (model_training/data/
+ *     utils.py:73-115, float64 then truncation to int32; x2 is computed from the already clipped x1, so a box left of the frame
+ *     is shifted, not cut); extend_h = (left, right, top, bottom) fractions as extend_bbox takes them.  A record is invalid
+ *     (valid = 0: scale 1, new_h = new_w = 0, zero paddings, an all-padding input image) when its frame index is outside
+ *     [0, F), its crop is empty, or a letter-boxed side rounds to 0 pixels (cv2.resize refuses that size, so the reference
+ *     cannot process the crop either).
+ *   dad3d_preprocess_rois  frames_d [F,H,W,3] uint8 RGB -> out_d [R,3,img_size,img_size] fp32: the letter-box of
+ *     dad3d_preprocess on each record's crop, read in place with the frame's row pitch (bilinear taps clamp at the crop's
+ *     border), bit-exact with cv2 on frame[y:y+h, x:x+w].  R <= 65535.
+ *   dad3d_readjust_rois  FaceMeshPredictor._get_predictions' read-back (predictor.py:117-123,141-176) plus the move into frame
+ *     pixels, per head, from the encoder's params_d [R,num_params] and landmarks_d [R,num_landmarks,2] (in [0,1] units):
+ *     params_out_d [R,num_params] = readjust_3dmm_to_the_input_image in fp32 (scale at scale_index, translation at
+ *     translation_index .. +2), then translation xy += [x, y] * 2 / img_size (the arithmetic of HeadMesh.adjust_3dmm_to_paddings,
+ *     head_mesh.py:48-60) and translation z = 0 (the in-place side effect of reprojected_vertices, head_mesh.py:41);
+ *     points_d [R,num_landmarks,2] int64 = readjust_landmarks_to_the_input_image(clip(lm * 256, 0, 256)) + [x, y], with the
+ *     reference's dtypes (fp32 multiply and clip, float64 subtract and divide, truncation).  params_out_d may be params_d. */
+typedef struct dad3d_roi {
+  int32_t x, y, w, h;             /* the crop, in frame pixels */
+  int32_t frame, valid;
+  int32_t new_h, new_w;           /* py3round(side * scale): the letter-boxed size */
+  int32_t pre_top, pre_left;      /* PadIfNeeded offsets of the letter-box (pre-processing) */
+  int32_t post_top, post_left;    /* calculate_paddings(new_h, new_w)[0], [2] (post-processing, predictor.py:117-123) */
+  double scale;                   /* img_size / double(max(h, w)) */
+  double inv_scale_x, inv_scale_y;  /* cv::resize's 1 / (new_w / w), 1 / (new_h / h) */
+} dad3d_roi;
+DAD3D_API int dad3d_roi_setup(const int32_t* boxes_d, const int32_t* frame_index_d, int32_t R, int32_t F, int32_t H, int32_t W,
+                              int32_t img_size, const double* extend_h, dad3d_roi* rois_d, dad3d_stream stream);
+DAD3D_API int dad3d_preprocess_rois(const uint8_t* frames_d, int32_t H, int32_t W, const dad3d_roi* rois_d, int32_t R,
+                                    int32_t img_size, const float* mean255_h, const float* inv_std255_h, float* out_d,
+                                    dad3d_stream stream);
+DAD3D_API int dad3d_readjust_rois(const float* params_d, const float* landmarks_d, const dad3d_roi* rois_d, int32_t R,
+                                  int32_t num_params, int32_t num_landmarks, int32_t scale_index, int32_t translation_index,
+                                  int32_t img_size, float* params_out_d, int64_t* points_d, dad3d_stream stream);
+
 /* Live timing of the dominant kernel (the wgmma tile engine) for bench.py's roofline: while on, every conv / linear
  * launch is bracketed by CUDA events on the launching stream.  profile_read synchronises those events and returns their
  * summed duration, the launch count and the ALGORITHMIC FLOPs (2 * true MACs, one product per MAC, no padding) of the
