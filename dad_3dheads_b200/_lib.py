@@ -76,6 +76,9 @@ SIGNATURES = {
     "dad3d_rasterize_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]),
+    "dad3d_rasterize_frames": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                         C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_vertex_normals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "dad3d_comm_unique_id": (C.c_int, [C.c_void_p]),
     "dad3d_comm_init": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),

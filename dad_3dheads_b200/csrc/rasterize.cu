@@ -10,6 +10,10 @@
 //   * both passes run over a batch of heads that share one triangle list and colour table (PNCC, depth and triangle-index
 //     maps of a whole predict_batch); each head has its own key words, so a head's result does not depend on the batch.
 //     dad3d_rasterize is the one-head call.
+//   * with a head -> image map (dad3d_rasterize_frames) several heads share one image's key words: the key's low word is
+//     ~(head * ntri + triangle), so one atomicMax keeps the nearest surface and, on an exact tie, the lower (head, triangle)
+//     pair -- the reference's loop over the union mesh of the image's heads in head order.  Pass 2 then runs over
+//     (pixel, image) and decodes head and triangle from the winner.  Without a map, image = head and the low word is ~triangle.
 //   * vertex normals accumulate the un-normalised face normals of the incident triangles in ascending triangle order (caller-built
 //     CSR adjacency), the order of the reference's scatter loop.
 // Integer / float HBM-bound work; no tensor cores.
@@ -63,14 +67,21 @@ __device__ __forceinline__ TriSetup load_tri(const float* __restrict__ v, const 
 }
 
 // pass 1: one thread per (triangle, head) walks the triangle's bounding box.  Heads run along grid y, strided by gridDim.y so
-// that batches past the 65 535 grid-y limit loop; every head offset is 64-bit.
+// that batches past the 65 535 grid-y limit loop; every head offset is 64-bit.  image_of_head (NULL: head b draws into image
+// b) sends a head's keys to its image; a head mapped outside [0, n_images) draws nothing.
 __global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int batch, const int* __restrict__ tris, int ntri,
-                                  int h, int w, int negate_z, const float* __restrict__ depth_in,
-                                  unsigned long long* __restrict__ key) {
+                                  int h, int w, int negate_z, const int* __restrict__ image_of_head, int n_images,
+                                  const float* __restrict__ depth_in, unsigned long long* __restrict__ key) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= ntri) return;
   const long long hw = static_cast<long long>(h) * w;
   for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    const int img = image_of_head ? image_of_head[b] : b;
+    if (img < 0 || img >= n_images) continue;
+    // the tie-break word: the triangle, or with a map the (head, triangle) pair, which the caller keeps below 2^32 - 1
+    const unsigned int rank = image_of_head ? static_cast<unsigned int>(b) * static_cast<unsigned int>(ntri) +
+                                                  static_cast<unsigned int>(i)
+                                            : static_cast<unsigned int>(i);
     TriSetup s = load_tri(verts + static_cast<long long>(b) * nv * 3, tris, i);
     if (negate_z) { s.d0 = -s.d0; s.d1 = -s.d1; s.d2 = -s.d2; }
     const int x_min = max(static_cast<int>(ceilf(fminf(s.p0x, fminf(s.p1x, s.p2x)))), 0);
@@ -78,8 +89,8 @@ __global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int b
     const int y_min = max(static_cast<int>(ceilf(fminf(s.p0y, fminf(s.p1y, s.p2y)))), 0);
     const int y_max = min(static_cast<int>(floorf(fmaxf(s.p0y, fmaxf(s.p1y, s.p2y)))), h - 1);
     if (x_max < x_min || y_max < y_min) continue;
-    const float* dh = depth_in ? depth_in + b * hw : nullptr;
-    unsigned long long* kh = key + b * hw;
+    const float* dh = depth_in ? depth_in + img * hw : nullptr;
+    unsigned long long* kh = key + img * hw;
     for (int y = y_min; y <= y_max; ++y)
       for (int x = x_min; x <= x_max; ++x) {
         float wt[3];
@@ -90,7 +101,7 @@ __global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int b
           if (d > (dh ? dh[pix] : -1e8f)) {                       // Sim3DR.py:22 initialises the buffer to -1e8
             // d + 0 maps -0 to +0 (and nothing else): the sequential z-test sees -0 and +0 as a tie, the lower index keeps it
             const unsigned long long k = (static_cast<unsigned long long>(orderable(radd(d, 0.0f))) << 32) |
-                                         static_cast<unsigned long long>(0xFFFFFFFFu - static_cast<unsigned int>(i));
+                                         static_cast<unsigned long long>(0xFFFFFFFFu - rank);
             atomicMax(&kh[pix], k);
           }
         }
@@ -98,21 +109,27 @@ __global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int b
   }
 }
 
-// pass 2: one thread per (pixel, head) shades the winning triangle; tri_index gets the winner or -1 in depth-buffer rows
-__global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, int batch, const int* __restrict__ tris,
-                                      const float* __restrict__ colors, int h, int w, int c, int reverse, int negate_z,
-                                      const unsigned long long* __restrict__ key, unsigned char* __restrict__ image,
-                                      float* __restrict__ depth, int* __restrict__ tri_index) {
+// pass 2: one thread per (pixel, image) shades the winning triangle; tri_index gets the winner or -1 in depth-buffer rows.
+// mapped != 0: the key names (head, triangle) as head * ntri + triangle, and head_index gets the head or -1.
+__global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, int n_images, const int* __restrict__ tris,
+                                      int ntri, int mapped, const float* __restrict__ colors, int h, int w, int c, int reverse,
+                                      int negate_z, const unsigned long long* __restrict__ key,
+                                      unsigned char* __restrict__ image, float* __restrict__ depth, int* __restrict__ tri_index,
+                                      int* __restrict__ head_index) {
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
   const long long hw = static_cast<long long>(h) * w;
   if (pix >= hw) return;
   const int y = pix / w, x = pix - y * w;
   const int yo = reverse ? (h - 1 - y) : y;
-  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
-    const long long at = b * hw + pix;
+  for (int m = blockIdx.y; m < n_images; m += gridDim.y) {
+    const long long at = m * hw + pix;
     const unsigned long long k = key[at];
-    const int i = k == 0ull ? -1 : static_cast<int>(0xFFFFFFFFu - static_cast<unsigned int>(k & 0xFFFFFFFFull));
+    const unsigned int rank = 0xFFFFFFFFu - static_cast<unsigned int>(k & 0xFFFFFFFFull);
+    const int b = k == 0ull ? -1 : (mapped ? static_cast<int>(rank / static_cast<unsigned int>(ntri)) : m);
+    const int i = k == 0ull ? -1 : (mapped ? static_cast<int>(rank - static_cast<unsigned int>(b) * ntri)
+                                           : static_cast<int>(rank));
     if (tri_index) tri_index[at] = i;
+    if (head_index) head_index[at] = b;
     if (i < 0) continue;
     const float* vh = verts + static_cast<long long>(b) * nv * 3;
     TriSetup s = load_tri(vh, tris, i);
@@ -121,7 +138,7 @@ __global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, i
     point_weight(wt, static_cast<float>(x), static_cast<float>(y), s.p0x, s.p0y, s.p1x, s.p1y, s.p2x, s.p2y);
     if (depth) depth[at] = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
     if (!image) continue;
-    unsigned char* px = image + (b * hw + static_cast<long long>(yo) * w + x) * c;
+    unsigned char* px = image + (m * hw + static_cast<long long>(yo) * w + x) * c;
     for (int ch = 0; ch < c; ++ch) {
       const float pc = radd(radd(rmul(wt[0], colors[c * s.i0 + ch]), rmul(wt[1], colors[c * s.i1 + ch])), rmul(wt[2], colors[c * s.i2 + ch]));
       // (unsigned char)((1 - alpha) * image + alpha * 255 * p_color) with alpha = 1
@@ -160,32 +177,69 @@ using namespace dad3d;
 
 extern "C" {
 
+}  // extern "C"
+
+namespace {
+
+// both entries: `batch` heads drawn into `n_images` images; image_of_head_d NULL is the identity map (n_images = batch)
+int rasterize_mapped(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                     const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
+                     const int32_t* image_of_head_d, int32_t n_images, uint8_t* image_d, float* depth_d,
+                     int32_t* tri_index_d, int32_t* head_index_d, unsigned long long* key_ws_d, dad3d_stream stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const size_t hw = static_cast<size_t>(h) * w;
+  if (n_images == 0) return DAD3D_OK;
+  if (batch == 0 || ntri == 0) {                     // nothing covers any pixel: image and depth stay, the indices are all -1
+    if (tri_index_d) DAD3D_CUDA_OK(cudaMemsetAsync(tri_index_d, 0xFF, sizeof(int32_t) * hw * n_images, stream));
+    if (head_index_d) DAD3D_CUDA_OK(cudaMemsetAsync(head_index_d, 0xFF, sizeof(int32_t) * hw * n_images, stream));
+    return DAD3D_OK;
+  }
+  DAD3D_CUDA_OK(cudaMemsetAsync(key_ws_d, 0, sizeof(unsigned long long) * hw * n_images, stream));
+  const unsigned int gy = static_cast<unsigned int>(batch < 65535 ? batch : 65535);
+  raster_tri_kernel<<<dim3((ntri + 127) / 128, gy), 128, 0, stream>>>(vertices_d, nv, batch, triangles_d, ntri, h, w,
+                                                                       negate_z, image_of_head_d, n_images, depth_d,
+                                                                       key_ws_d);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  const unsigned int gm = static_cast<unsigned int>(n_images < 65535 ? n_images : 65535);
+  raster_resolve_kernel<<<dim3(static_cast<unsigned int>((hw + 255) / 256), gm), 256, 0, stream>>>(
+      vertices_d, nv, n_images, triangles_d, ntri, image_of_head_d ? 1 : 0, colors_d, h, w, c, reverse, negate_z, key_ws_d,
+      image_d, depth_d, tri_index_d, head_index_d);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
                           const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
                           uint8_t* image_d, float* depth_d, int32_t* tri_index_d, unsigned long long* key_ws_d,
-                          dad3d_stream stream_) {
+                          dad3d_stream stream) {
   DAD3D_REQUIRE(vertices_d && (triangles_d || ntri == 0) && key_ws_d, "null pointer");
   DAD3D_REQUIRE(!image_d || colors_d, "image_d needs colors_d");
   DAD3D_REQUIRE(batch >= 0 && nv > 0 && ntri >= 0 && h > 0 && w > 0 && c > 0 && static_cast<long long>(h) * w < (1ll << 31),
                 "shape");
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  const size_t hw = static_cast<size_t>(h) * w;
-  if (batch == 0) return DAD3D_OK;
-  if (ntri == 0) {                                   // nothing covers any pixel: image and depth stay, tri_index is all -1
-    if (tri_index_d) DAD3D_CUDA_OK(cudaMemsetAsync(tri_index_d, 0xFF, sizeof(int32_t) * hw * batch, stream));
-    return DAD3D_OK;
-  }
-  DAD3D_CUDA_OK(cudaMemsetAsync(key_ws_d, 0, sizeof(unsigned long long) * hw * batch, stream));
-  const unsigned int gy = static_cast<unsigned int>(batch < 65535 ? batch : 65535);
-  raster_tri_kernel<<<dim3((ntri + 127) / 128, gy), 128, 0, stream>>>(vertices_d, nv, batch, triangles_d, ntri, h, w,
-                                                                       negate_z, depth_d, key_ws_d);
-  count_launch();
-  DAD3D_CUDA_OK(cudaGetLastError());
-  raster_resolve_kernel<<<dim3(static_cast<unsigned int>((hw + 255) / 256), gy), 256, 0, stream>>>(
-      vertices_d, nv, batch, triangles_d, colors_d, h, w, c, reverse, negate_z, key_ws_d, image_d, depth_d, tri_index_d);
-  count_launch();
-  DAD3D_CUDA_OK(cudaGetLastError());
-  return DAD3D_OK;
+  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, c, h, w, reverse, negate_z, nullptr, batch,
+                          image_d, depth_d, tri_index_d, nullptr, key_ws_d, stream);
+}
+
+int dad3d_rasterize_frames(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                           const float* colors_d, int32_t c, const int32_t* image_of_head_d, int32_t n_images, int32_t h,
+                           int32_t w, int32_t negate_z, uint8_t* image_d, float* depth_d, int32_t* tri_index_d,
+                           int32_t* head_index_d, unsigned long long* key_ws_d, dad3d_stream stream) {
+  DAD3D_REQUIRE(((vertices_d && image_of_head_d) || batch == 0) && (triangles_d || ntri == 0) && key_ws_d, "null pointer");
+  DAD3D_REQUIRE(!image_d || colors_d, "image_d needs colors_d");
+  DAD3D_REQUIRE(batch >= 0 && nv > 0 && ntri >= 0 && n_images >= 0 && h > 0 && w > 0 && c > 0 &&
+                    static_cast<long long>(h) * w < (1ll << 31),
+                "shape");
+  // the key's low word holds ~(head * ntri + triangle): every pair must stay below 2^32 - 1
+  DAD3D_REQUIRE(static_cast<unsigned long long>(batch) * static_cast<unsigned long long>(ntri) <= 0xFFFFFFFEull,
+                "batch * ntri exceeds 2^32 - 2");
+  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, c, h, w, 0, negate_z, image_of_head_d, n_images,
+                          image_d, depth_d, tri_index_d, head_index_d, key_ws_d, stream);
 }
 
 int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri, uint8_t* image_d,

@@ -6,7 +6,8 @@ stages and their helper names, so ``demo.py`` / ``demo_utils.py`` code written a
 What changes is where the arithmetic runs: ``self.model`` is the CUDA encoder (csrc/encoder.cu) instead of a TorchScript
 module, and ``self.head_mesh`` decodes on the GPU (csrc/flame.cu), once instead of twice per image.
 ``predict_batch`` is the batched, device-resident entry point the reference does not have (SURVEY §8b); with ``render`` it
-also draws the PNCC, depth and triangle-index maps of every head (rasterizer.PnccRenderer) inside the same step.
+also draws the PNCC, depth and triangle-index maps of every head (rasterizer.PnccRenderer) inside the same step, and with
+``boxes`` plus ``frame_render`` the same maps of every whole frame, all its heads in one z-buffer.
 """
 from __future__ import annotations
 
@@ -32,6 +33,7 @@ _FILENAME = "dad_3dheads.trcd"
 _MEAN = (0.485, 0.456, 0.406)
 _STD = (0.229, 0.224, 0.225)
 RENDER_KEYS = ("pncc", "depth", "tri_index")
+FRAME_RENDER_KEYS = ("pncc", "depth", "tri_index", "head_index")    # predict_batch(boxes=, frame_render=) -> "frame_<key>"
 
 DEFAULT_CONFIG = {                                   # == the reference's dad_3dnet.yaml
     "model_path": ".dad_checkpoints/dad_3dheads.trcd",
@@ -283,6 +285,28 @@ class FaceMeshPredictor:
             raise ValueError("render needs to_2d=False: the renderer takes the projected vertices with their depth")
         return keys
 
+    @staticmethod
+    def _frame_render_keys(frame_render, to_2d: bool, boxes) -> Tuple[str, ...]:
+        """``frame_render`` as a canonical tuple (the order of FRAME_RENDER_KEYS), validated against ``to_2d`` and ``boxes``."""
+        if frame_render is None:
+            return ()
+        if isinstance(frame_render, str):
+            frame_render = (frame_render,)
+        unknown = set(frame_render) - set(FRAME_RENDER_KEYS)
+        if unknown:
+            raise ValueError(f"frame_render: unknown maps {sorted(unknown)}; choose from {FRAME_RENDER_KEYS}")
+        keys = tuple(k for k in FRAME_RENDER_KEYS if k in frame_render)
+        if keys and boxes is None:
+            raise ValueError("frame_render needs boxes: it draws the heads of each box into its frame")
+        if keys and to_2d:
+            raise ValueError("frame_render needs to_2d=False: the renderer takes the projected vertices with their depth")
+        return keys
+
+    def _pncc_renderer(self) -> PnccRenderer:
+        if self._renderer is None:                           # uploads its tables once (graph-capture safe afterwards)
+            self._renderer = PnccRenderer(self.device)
+        return self._renderer
+
     def _check_rois(self, frames, boxes, frame_index) -> Tuple[Tensor, Optional[Tensor]]:
         """Validates the frames + boxes arguments before anything is launched -> (boxes, frame_index) as tensors."""
         if not (isinstance(frames, Tensor) and frames.dtype == torch.uint8 and frames.ndim == 4 and frames.shape[3] == 3):
@@ -308,7 +332,8 @@ class FaceMeshPredictor:
             raise ValueError("boxes need the released 3DMM layout (one scale, three translation parameters)")
         return boxes, frame_index
 
-    def _predict_rois(self, frames, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode) -> Dict[str, Tensor]:
+    def _predict_rois(self, frames, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
+                      frame_render=()) -> Dict[str, Tensor]:
         """predict_batch with boxes: crop geometry, pre-processing and read-back in csrc/roi.cu, no host synchronisation."""
         boxes, frame_index = self._check_rois(frames, boxes, frame_index)
         ext = np.array(extend_sides(extend), dtype=np.float64)
@@ -345,11 +370,18 @@ class FaceMeshPredictor:
         if landmark_subset is not None:
             dec = self.head_mesh.flame.decoder(self.device)
             out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
+        if frame_render:
+            frame_of_head = torch.where(out["valid"], fields[:, 4], -1)            # invalid boxes draw nothing
+            maps = self._pncc_renderer().render_frames(proj, frame_of_head, F, (H, W), pncc="pncc" in frame_render,
+                                                       depth="depth" in frame_render,
+                                                       tri_index="tri_index" in frame_render,
+                                                       head_index="head_index" in frame_render)
+            out.update({f"frame_{k}": t for k, t in maps.items()})
         return out
 
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                       fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                      extend=0.0) -> Dict[str, Tensor]:
+                      extend=0.0, frame_render=None) -> Dict[str, Tensor]:
         """images: [B,3,256,256] fp32 already letter-boxed + normalised, or raw RGB as the reference's ``__call__`` takes it:
         one [B,H,W,3] uint8 tensor / a list of HxWx3 uint8 images (letter-boxed + normalised on the GPU, bit-identical to
         the reference's albumentations pipeline); host or device.  All outputs stay on the GPU:
@@ -369,12 +401,24 @@ class FaceMeshPredictor:
         "projected_vertices" / "landmarks_<subset>" decoded from those parameters; plus "crop_boxes" [R,4] int32 and
         "valid" [R] bool.  A box is invalid when its frame index is out of range, its crop is empty, or a side of its
         letter-box rounds to 0 pixels; its outputs are finite but meaningless.  Nothing waits for the device, so boxes
-        computed on the GPU are consumed directly.  At most 65 535 boxes per call; ``render`` is not supported."""
+        computed on the GPU are consumed directly.  At most 65 535 boxes per call; ``render`` is not supported.
+
+        ``frame_render`` (with ``boxes`` and ``to_2d=False``): a subset of ("pncc", "depth", "tri_index", "head_index") adds
+        those maps of every whole frame, all its valid boxes' heads drawn from "projected_vertices" into one image and one
+        z-buffer (:meth:`~dad_3dheads_b200.rasterizer.PnccRenderer.render_frames`): "frame_pncc" [F,H,W,3] uint8,
+        "frame_depth" [F,H,W] fp32 (-z; -1e8 for background), "frame_tri_index" [F,H,W] int32 (the triangle within its
+        head) and "frame_head_index" [F,H,W] int32 (the box), -1 for background.  A frame equals the reference's
+        ``PNCCEstimator()(frame, {"3dmm_params": p})`` run for its boxes' frame-space parameters one after the other in box
+        order on the same buffers: the nearest head wins, an exact depth tie goes to the earlier box, invalid boxes draw
+        nothing.  The reference's ``with_background=True`` overlay is, exactly,
+        ``torch.where(out["frame_head_index"][..., None] >= 0, out["frame_pncc"], frames)``."""
         render = self._render_keys(render, to_2d)
+        frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
         if boxes is not None:
             if render:
                 raise ValueError("render is not supported together with boxes")
-            return self._predict_rois(images, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode)
+            return self._predict_rois(images, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
+                                      frame_render)
         if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
             x = self.preprocess_batch(images)
         else:
@@ -387,9 +431,7 @@ class FaceMeshPredictor:
             dec = self.head_mesh.flame.decoder(self.device)
             out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
         if render:
-            if self._renderer is None:                       # uploads its tables once (graph-capture safe afterwards)
-                self._renderer = PnccRenderer(self.device)
-            out.update(self._renderer(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
+            out.update(self._pncc_renderer()(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
                                       tri_index="tri_index" in render))
         return out
 
@@ -398,11 +440,11 @@ class FaceMeshPredictor:
         dec = self.head_mesh.flame.decoder(self.device)
         return (self.model.ws_generation, dec.ws_generation)
 
-    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None):
+    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None, frame_render=()):
         """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph.
         ``rois`` = (static boxes [R,4] int32, static frame index [R] int32, extend): the graph reads the boxes from those
         buffers on every replay."""
-        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2]) if rois is not None else {}
+        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2], frame_render=frame_render) if rois is not None else {}
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
@@ -430,7 +472,7 @@ class FaceMeshPredictor:
 
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                               fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                              extend=0.0) -> Dict[str, Tensor]:
+                              extend=0.0, frame_render=None) -> Dict[str, Tensor]:
         """:meth:`predict_batch` replayed from a CUDA graph (one graph per input shape / dtype / option set): the ~110 kernel
         launches of a step become one graph launch, which removes the launch gaps between the many sub-20 us layers.
         ``images`` is copied into the graph's static input buffer (host or device source); the returned tensors are the
@@ -441,10 +483,11 @@ class FaceMeshPredictor:
         re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced.
 
         With ``boxes`` (see :meth:`predict_batch`) the boxes and frame indices are copied into static buffers as well: one
-        graph serves every box set of the same frame shape, box count and ``extend``."""
+        graph serves every box set of the same frame shape, box count, ``extend`` and ``frame_render``."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
         render = self._render_keys(render, to_2d)
-        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render)
+        frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
+        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render, frame_render)
         if boxes is not None:
             if render:
                 raise ValueError("render is not supported together with boxes")
@@ -460,7 +503,7 @@ class FaceMeshPredictor:
             rois = self._roi_buffers(int(boxes.shape[0]), extend) if boxes is not None else None
             if rois is not None:
                 self._fill_rois(rois, boxes, frame_index)
-            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois)
+            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois, frame_render)
             ent = (graph, static_in, out, gen, rois)
             self._graphs[key] = ent
         graph, static_in, out, _, rois = ent
@@ -472,7 +515,8 @@ class FaceMeshPredictor:
 
     def open_stream(self, shape, dtype=torch.uint8, **kw) -> "BatchStream":
         """A double-buffered pipeline over :meth:`predict_batch` for a fixed batch signature -- see :class:`BatchStream`.
-        ``rois=R`` (with optional ``extend``): ``shape`` is that of the frames, and every submit brings R boxes."""
+        ``rois=R`` (with optional ``extend`` and ``frame_render``): ``shape`` is that of the frames, and every submit brings R
+        boxes."""
         return BatchStream(self, shape, dtype, **kw)
 
 
@@ -487,14 +531,15 @@ class BatchStream:
     batches have been submitted.  ``render`` is passed to ``predict_batch`` (with ``to_2d=False``); list the maps in
     ``keys`` to have them copied to the host like the other outputs.  With ``rois=R`` each batch is frames plus R boxes
     (``predict_batch``'s ``boxes``): ``submit(frames, boxes=, frame_index=)`` copies the boxes on the copy stream together with
-    the frames; "crop_boxes" and "valid" may be listed in ``keys``.
+    the frames; "crop_boxes" and "valid" may be listed in ``keys``, and with ``frame_render`` (passed to ``predict_batch``)
+    the "frame_<map>" outputs too.
     """
 
     def __init__(self, predictor: FaceMeshPredictor, shape, dtype=torch.uint8, landmark_subset: Optional[str] = "445",
                  to_2d: bool = True, fast_decode: bool = True, depth: int = 2, render=None,
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
                  group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None, rois=None,
-                 extend=0.0):
+                 extend=0.0, frame_render=None):
         self.pred = predictor
         dev = predictor.device
         self.device = dev
@@ -511,13 +556,14 @@ class BatchStream:
         self._args = (landmark_subset, to_2d, fast_decode, predictor._render_keys(render, to_2d))
         if rois is not None and self._args[3]:
             raise ValueError("render is not supported together with boxes")
+        self._frame_render = predictor._frame_render_keys(frame_render, to_2d, rois)
         self.rois = rois
         self.slots = []
         with torch.cuda.device(dev):
             for _ in range(self.depth):
                 static_in = torch.zeros(tuple(shape), dtype=dtype, device=dev)
                 roi_bufs = predictor._roi_buffers(int(rois), extend) if rois is not None else None
-                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs)
+                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs, self._frame_render)
                 slot = {"in": static_in, "rois": roi_bufs, "graph": graph, "out": out, "gen": gen, "busy": False,
                         "h2d": torch.cuda.Event(), "done": torch.cuda.Event(), "comm_done": torch.cuda.Event(),
                         "d2h": torch.cuda.Event(), "gathered": {}, "host": {}}
@@ -549,7 +595,7 @@ class BatchStream:
         s = self.slots[self._head]
         if s["gen"] != self.pred._ws_generation():           # scratch reallocated by another caller: re-capture this slot
             torch.cuda.synchronize(self.device)
-            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"])
+            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"], self._frame_render)
         with torch.cuda.stream(self.copy_in):
             self.copy_in.wait_event(s["done"])               # the previous replay of this slot has consumed its input
             s["in"].copy_(images, non_blocking=True)

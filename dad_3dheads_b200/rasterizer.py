@@ -4,7 +4,9 @@ the reference's ``inference/pncc_estimator.py`` through ``compat/Sim3DR``.  No C
 
 ``rasterize_batch`` and ``PnccRenderer`` are the batched, device-resident form: B heads of one topology per call, device
 tensors in and out, no host synchronisation (so they run inside a captured CUDA graph); every head equals, bit for bit, what
-``rasterize`` gives for that head alone."""
+``rasterize`` gives for that head alone.  With a head -> image map (``rasterize_batch(image_of_head=, num_images=)``,
+``PnccRenderer.render_frames``) several heads share one image and one z-buffer, as when a caller of the reference draws the
+heads of a whole frame one after the other into the same buffers."""
 from __future__ import annotations
 
 import os
@@ -97,7 +99,8 @@ def _check_triangles(triangles: torch.Tensor, nv: int) -> None:
 
 def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Optional[torch.Tensor] = None, *, height: int,
                     width: int, image: Optional[torch.Tensor] = None, depth: bool = True, tri_index: bool = True,
-                    reverse: bool = False, negate_z: bool = False) -> Dict[str, torch.Tensor]:
+                    reverse: bool = False, negate_z: bool = False, image_of_head: Optional[torch.Tensor] = None,
+                    num_images: Optional[int] = None, head_index: bool = True) -> Dict[str, torch.Tensor]:
     """Z-buffer rendering of B heads that share one mesh topology, on the GPU (``dad3d_rasterize_batch``).
 
     vertices [B,nv,3] float32 (x, y in pixels, z = depth, larger wins; with ``negate_z`` -z is the depth), triangles [ntri,3]
@@ -105,7 +108,14 @@ def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Opt
     "image" [B,height,width,C] uint8 (when ``colors`` is given: zeros, or a copy of ``image``, with the heads drawn over it;
     ``reverse`` flips its rows), "depth" [B,height,width] float32 (-1e8 where no triangle covers the pixel), "tri_index"
     [B,height,width] int32 (the winning triangle, -1 for background, in depth-map rows).  Runs on the current stream without
-    a host synchronisation, except the first bounds check of a ``triangles`` tensor."""
+    a host synchronisation, except the first bounds check of a ``triangles`` tensor.
+
+    ``image_of_head`` ([B] int32 on the device) and ``num_images`` draw the heads into ``num_images`` shared images
+    (``dad3d_rasterize_frames``): head b goes to image ``image_of_head[b]``, and a head mapped outside [0, num_images) draws
+    nothing.  Every map is then [num_images, ...], and "head_index" [num_images,height,width] int32 names the winning head
+    (-1 for background; ``head_index=False`` leaves it out).  Each image equals the reference's rasteriser run over its
+    heads one after the other in head order with carried buffers: the nearest surface wins, and an exact depth tie goes to
+    the lower (head, triangle) pair.  ``reverse`` is not available with a map."""
     if vertices.ndim != 3 or vertices.shape[2] != 3 or vertices.dtype != torch.float32 or not vertices.is_cuda:
         raise ValueError("vertices must be a [B,nv,3] float32 CUDA tensor")
     if triangles.ndim != 2 or triangles.shape[1] != 3 or triangles.dtype != torch.int32 or triangles.device != vertices.device:
@@ -115,6 +125,21 @@ def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Opt
     height, width = int(height), int(width)
     if nv == 0 or height <= 0 or width <= 0 or height * width >= 1 << 31:
         raise ValueError(f"bad shape: nv={nv}, height={height}, width={width}")
+    mapped = image_of_head is not None
+    if mapped != (num_images is not None):
+        raise ValueError("image_of_head and num_images go together")
+    n_out = B
+    if mapped:
+        if image_of_head.shape != (B,) or image_of_head.dtype != torch.int32 or image_of_head.device != dev:
+            raise ValueError(f"image_of_head must be a [{B}] int32 tensor on the vertices' device")
+        if reverse:
+            raise ValueError("reverse is not available with image_of_head")
+        n_out = int(num_images)
+        if n_out < 0:
+            raise ValueError(f"num_images must be >= 0, got {n_out}")
+        if B * int(triangles.shape[0]) > 2 ** 32 - 2:
+            raise ValueError(f"{B} heads x {int(triangles.shape[0])} triangles exceed 2^32 - 2 (head, triangle) pairs")
+        image_of_head = image_of_head.contiguous()
     vertices = vertices.contiguous()
     triangles = triangles.contiguous()
     _check_triangles(triangles, nv)
@@ -126,26 +151,35 @@ def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Opt
         colors = colors.contiguous()
         c = int(colors.shape[1])
         if image is None:
-            out["image"] = torch.zeros(B, height, width, c, dtype=torch.uint8, device=dev)
+            out["image"] = torch.zeros(n_out, height, width, c, dtype=torch.uint8, device=dev)
         else:
-            if tuple(image.shape) != (B, height, width, c) or image.dtype != torch.uint8:
-                raise ValueError(f"image must be [{B},{height},{width},{c}] uint8")
+            if tuple(image.shape) != (n_out, height, width, c) or image.dtype != torch.uint8:
+                raise ValueError(f"image must be [{n_out},{height},{width},{c}] uint8")
             out["image"] = image.to(dev, copy=True).contiguous()
     elif image is not None:
         raise ValueError("image needs colors")
     if depth:
-        out["depth"] = torch.full((B, height, width), -1e8, dtype=torch.float32, device=dev)     # Sim3DR.py:22
+        out["depth"] = torch.full((n_out, height, width), -1e8, dtype=torch.float32, device=dev)     # Sim3DR.py:22
     if tri_index:
-        out["tri_index"] = torch.empty(B, height, width, dtype=torch.int32, device=dev)
-    key = torch.empty(B * height * width, dtype=torch.int64, device=dev)       # caching allocator: capture-safe
+        out["tri_index"] = torch.empty(n_out, height, width, dtype=torch.int32, device=dev)
+    if mapped and head_index:
+        out["head_index"] = torch.empty(n_out, height, width, dtype=torch.int32, device=dev)
+    key = torch.empty(n_out * height * width, dtype=torch.int64, device=dev)   # caching allocator: capture-safe
     ptr = lambda name: out[name].data_ptr() if name in out else None           # noqa: E731
     lib = _lib.load()
     with torch.cuda.device(dev):
-        _lib.check(lib.dad3d_rasterize_batch(vertices.data_ptr(), nv, B, triangles.data_ptr(), int(triangles.shape[0]),
-                                             colors.data_ptr() if colors is not None else None, c, height, width,
-                                             1 if reverse else 0, 1 if negate_z else 0, ptr("image"), ptr("depth"),
-                                             ptr("tri_index"), key.data_ptr(), torch.cuda.current_stream(dev).cuda_stream),
-                   "dad3d_rasterize_batch")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        cptr = colors.data_ptr() if colors is not None else None
+        if mapped:
+            _lib.check(lib.dad3d_rasterize_frames(vertices.data_ptr(), nv, B, triangles.data_ptr(), int(triangles.shape[0]),
+                                                  cptr, c, image_of_head.data_ptr(), n_out, height, width,
+                                                  1 if negate_z else 0, ptr("image"), ptr("depth"), ptr("tri_index"),
+                                                  ptr("head_index"), key.data_ptr(), stream), "dad3d_rasterize_frames")
+        else:
+            _lib.check(lib.dad3d_rasterize_batch(vertices.data_ptr(), nv, B, triangles.data_ptr(), int(triangles.shape[0]),
+                                                 cptr, c, height, width, 1 if reverse else 0, 1 if negate_z else 0,
+                                                 ptr("image"), ptr("depth"), ptr("tri_index"), key.data_ptr(), stream),
+                       "dad3d_rasterize_batch")
     return out
 
 
@@ -190,6 +224,30 @@ class PnccRenderer:
             raise ValueError(f"expected [B,{self.colors.shape[0]},3] vertices, got {tuple(projected_vertices_3d.shape)}")
         out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=size, width=size,
                               depth=depth, tri_index=tri_index, negate_z=True)
+        if pncc:
+            out["pncc"] = out.pop("image")
+        return out
+
+    def render_frames(self, projected_vertices_3d: torch.Tensor, frame_of_head: torch.Tensor, num_frames: int, size, *,
+                      pncc: bool = True, depth: bool = True, tri_index: bool = True,
+                      head_index: bool = True) -> Dict[str, torch.Tensor]:
+        """The frame form: B heads in the pixels of whole frames, drawn into ``num_frames`` frames of ``size`` = (H, W)
+        with one z-buffer per frame.  ``frame_of_head`` [B] int32 on the device names each head's frame; a head whose entry
+        is outside [0, num_frames) (e.g. -1 for an invalid box) draws nothing.  Returns {"pncc": [F,H,W,3] uint8, "depth":
+        [F,H,W] float32 (-z; -1e8 for background), "tri_index": [F,H,W] int32 (index into ``faces`` of the winning head),
+        "head_index": [F,H,W] int32 (the winning head)}, -1 for background in both index maps.
+
+        A frame equals the reference's ``PNCCEstimator()(frame, {"3dmm_params": p}, with_background=False)``
+        (inference/pncc_estimator.py:88-101) over its heads one after the other in head order, each drawing into the same
+        image and depth buffer: the nearest surface wins across heads, and an exact depth tie goes to the lower head.  The
+        reference's ``with_background=True`` overlay is ``torch.where(head_index[..., None] >= 0, pncc, frames)``, exactly,
+        since alpha = 1 overwrites every covered pixel."""
+        if projected_vertices_3d.ndim != 3 or projected_vertices_3d.shape[1:] != (self.colors.shape[0], 3):
+            raise ValueError(f"expected [B,{self.colors.shape[0]},3] vertices, got {tuple(projected_vertices_3d.shape)}")
+        height, width = (int(v) for v in size)
+        out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=height, width=width,
+                              depth=depth, tri_index=tri_index, negate_z=True, image_of_head=frame_of_head,
+                              num_images=num_frames, head_index=head_index)
         if pncc:
             out["pncc"] = out.pop("image")
         return out

@@ -314,6 +314,19 @@ DAD3D_API int dad3d_allgather_outputs(dad3d_comm* c, const void* send_d, void* r
  *     be NULL when image_d is, triangles_d when ntri = 0.  key_ws_d = batch*h*w 64-bit words of scratch.  Every head equals, bit for bit, a
  *     single-head call on that head.  batch = 0 launches nothing; ntri = 0 launches nothing and sets tri_index_d to -1.
  *     dad3d_rasterize is the batch = 1 call of these kernels.
+ *   dad3d_rasterize_frames: `batch` heads of one topology drawn into `n_images` shared images (several heads per whole
+ *     frame, one z-buffer per frame), with the same two kernels.  image_of_head_d [batch] int32 (device) names each head's
+ *     image; a head whose entry is outside [0, n_images) draws nothing (checked on the device, no host read).  Image m equals
+ *     the reference's _rasterize (Sim3DR/lib/rasterize_kernel.cpp:238-292, alpha = 1) called once on the union mesh of the
+ *     heads mapped to m in head order -- their vertices concatenated, each head's triangles offset by its vertex base -- which
+ *     is the reference's per-head call (inference/pncc_estimator.py:16-43,88-101) repeated in head order with the image and
+ *     depth buffer carried over.  So the nearest surface wins across heads, and an exact depth tie goes to the lower
+ *     (head, triangle) pair, head first.  Outputs, each may be NULL: image_d [n_images,h,w,c] uint8 and depth_d
+ *     [n_images,h,w] fp32 read-modify-write as in dad3d_rasterize_batch; tri_index_d [n_images,h,w] int32, the winning
+ *     triangle within its head; head_index_d [n_images,h,w] int32, the winning head; both -1 for background.  No reverse.
+ *     key_ws_d = n_images*h*w 64-bit words of scratch.  batch * ntri > 2^32 - 2 is DAD3D_ERR_INVALID (the key names a
+ *     pair in 32 bits).  batch = 0 or ntri = 0 launches nothing and sets the index maps to -1 (with batch = 0, vertices_d
+ *     and image_of_head_d may be NULL).
  *   dad3d_vertex_normals: normalised sum of the incident (un-normalised) face normals per vertex; adj_offsets_d [nv+1] /
  *     adj_triangles_d = CSR list of each vertex's triangles in ascending order (fixed per topology). */
 DAD3D_API int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri,
@@ -323,6 +336,11 @@ DAD3D_API int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t
                                     const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
                                     uint8_t* image_d, float* depth_d, int32_t* tri_index_d, unsigned long long* key_ws_d,
                                     dad3d_stream stream);
+DAD3D_API int dad3d_rasterize_frames(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d,
+                                     int32_t ntri, const float* colors_d, int32_t c, const int32_t* image_of_head_d,
+                                     int32_t n_images, int32_t h, int32_t w, int32_t negate_z, uint8_t* image_d, float* depth_d,
+                                     int32_t* tri_index_d, int32_t* head_index_d, unsigned long long* key_ws_d,
+                                     dad3d_stream stream);
 DAD3D_API int dad3d_vertex_normals(const float* vertices_d, const int32_t* triangles_d, const int32_t* adj_offsets_d,
                                    const int32_t* adj_triangles_d, int32_t nver, float* normals_d, dad3d_stream stream);
 
