@@ -515,7 +515,18 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     std::memset(&fit, 0, sizeof(fit));
     fit.nA = enc->P; fit.nB = enc->P; fit.block_n = w->block_n; fit.frag_epi = g.frag_epi;
     const bool narrow = w->has_b64 && (m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms || gemm_max_stages(fit) < 2);
-    const int block_n = narrow ? 64 : w->block_n;
+    // ping-pong consumers (tile_gemm.cuh) on 128 x 64 tiles: fragment-epilogue launches outside halo mode (and so outside
+    // clusters) whose 64-wide ring is at least two deep, with more than one product per k-block and at most
+    // kPingPongMaxKb k-blocks per tile.  Measured on H100 (profiles/README.md): in fp16x2 at batch 64 every such launch of
+    // up to 32 k-blocks ran faster or level, the 3x3 layers of 36 and 72 k-blocks slower; with one product per k-block
+    // (bf16, batch 512) ping-pong everywhere was slower, its main loop being bound by the operand bytes that 64-wide
+    // tiles raise.
+    constexpr int kPingPongMaxKb = 32;
+    const int kb64 = w->R * w->S * g.cin_blocks + (res_in_k ? 1 : src2 ? cin2 / kBlockK : 0);   // k-blocks at block_n 64
+    fit.block_n = 64;
+    g.pingpong = g.frag_epi && !halo && (w->block_n == 64 || w->has_b64) && gemm_max_stages(fit) >= 2 &&
+                 enc->n_mma > 1 && kb64 <= kPingPongMaxKb ? 1 : 0;
+    const int block_n = narrow || g.pingpong ? 64 : w->block_n;
     g.block_n = block_n;
     g.n_tiles = w->cout_pad / block_n;
     g.nA = enc->P; g.nB = enc->P;
@@ -560,7 +571,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
       const uint32_t es[4] = {1, static_cast<uint32_t>(s.stride), static_cast<uint32_t>(s.stride), 1};
       const uint16_t* basep = reinterpret_cast<const uint16_t*>(ti.ptr) + static_cast<size_t>(p) * ti.plane_elems();
       if (!make_tmap_16bit(&s.maps.a[p], basep, 4, dims, strides, box, es)) return DAD3D_ERR_CUDA;
-      s.maps.b[p] = (narrow || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];
+      s.maps.b[p] = (block_n != w->block_n || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];
     }
     if (res_in_k || src2) {
       const TensorInfo& tr = plan->tensors[s.res];
@@ -653,6 +664,14 @@ double conv_useful_flops(const Step& s) {
   return 2.0 * g.Nimg * rows * g.Wo * cout * cin * w->R * w->S;
 }
 
+// CTAs of a conv launch: one per SM at most, a whole number of clusters
+int conv_grid(const dad3d_encoder* enc, const GemmGeom& g) {
+  const int m_tiles_total = g.tiles_w * g.tiles_h * g.tiles_n;
+  const int csz = g.cl_m * g.cl_n;
+  if (csz > 1) return std::min(((m_tiles_total + g.cl_m - 1) / g.cl_m) * csz, (enc->num_sms / csz) * csz);
+  return std::min(m_tiles_total * g.n_tiles, enc->num_sms);
+}
+
 int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
   if (!enc->kernels_configured) {                  // function attributes are per device: remembered per handle
     DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConv>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
@@ -660,11 +679,8 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
     enc->kernels_configured = true;
   }
   const GemmGeom& g = s.geom;
-  const int m_tiles_total = g.tiles_w * g.tiles_h * g.tiles_n;
-  const int total = m_tiles_total * g.n_tiles;
-  int grid = std::min(total, enc->num_sms);
+  const int grid = conv_grid(enc, g);
   const int csz = g.cl_m * g.cl_n;
-  if (csz > 1) grid = std::min(((m_tiles_total + g.cl_m - 1) / g.cl_m) * csz, (enc->num_sms / csz) * csz);
   std::pair<cudaEvent_t, cudaEvent_t>* ev = nullptr;
   if (enc->profile) {
     if (enc->prof_used == enc->prof_events.size()) {
@@ -1180,6 +1196,14 @@ int dad3d_encoder_describe_plan(dad3d_encoder* enc, char* buf, size_t cap) {
       num("frag_epi", g.frag_epi); num("res_kb", g.res_kb); num("res_kind", g.res_kind); num("res_stride", g.res_stride);
       num("up2", s.up2); num("parity", s.parity); num("rowmap_n", g.rowmap_n); num("n_mma", g.n_mma); num("n_acc", g.n_acc);
       num("cout", s.w->cout); num("cin", s.w->cin); num("has_identity", s.w->has_identity ? 1 : 0);
+      const int grid = conv_grid(enc, g);
+      int tmin = 1 << 30, tmax = 0;
+      for (int b = 0; b < grid; ++b) {
+        const int t = gemm_cta_tiles(g, b, grid);
+        tmin = std::min(tmin, t);
+        tmax = std::max(tmax, t);
+      }
+      num("pingpong", g.pingpong); num("grid", grid); num("cta_tiles_min", tmin); num("cta_tiles_max", tmax);
       j += "\"rowmap\":[";
       for (int r = 0; r < g.rowmap_n; ++r) j += (r ? "," : "") + std::to_string(g.rowmap[r]);
       j += "],";

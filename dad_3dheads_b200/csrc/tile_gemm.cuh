@@ -33,7 +33,8 @@
 // The operand format (fp16 / bf16) is Epi::kBf16, a compile-time constant of the epilogue type.
 // Variants selected per launch in GemmGeom: halo (3x3 stride-1 convolutions: one halo patch per channel block feeds all nine
 // taps through shifted descriptors; separate weights ring), res_kb / res_kind (residual or second source on the K axis),
-// cl_m x cl_n multicast clusters.
+// cl_m x cl_n multicast clusters, and ping-pong consumers (GemmGeom::pingpong: each warpgroup owns whole 128 x 64 tiles and the
+// two take turns in the main loop, so one warpgroup's epilogue runs under the other's main loop; gemm_consumer_pingpong).
 #pragma once
 #include "ptx.cuh"
 
@@ -107,6 +108,10 @@ struct GemmGeom {
                                    // 1: row-tile persistent -- CTA b owns row tiles b, b+grid, ... and walks ALL column
                                    //    tiles of each (per-row-tile epilogue state is loaded once; all CTAs sweep the
                                    //    B operand in step, so it stays hot in L2)
+  int pingpong;                    // 1: PING-PONG consumers (fragment epilogue, block_n = 64, no halo, no cluster, stages >= 2):
+                                   // warpgroup w owns whole tiles -- positions w, w + 2, ... of the CTA's sequence -- and
+                                   // their main loops take turns, so one warpgroup's epilogue runs under the other's main
+                                   // loop (gemm_consumer_pingpong).  0: both warpgroups split every tile by rows.
 };
 
 struct GemmMaps {
@@ -162,31 +167,46 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmGeom& g, int m_tile, 
   return c;
 }
 
-// i-th tile of this CTA under the geometry's schedule; false when the CTA is out of work
-__device__ __forceinline__ bool tile_at(const GemmGeom& g, int i, TileCoord* tc) {
+// The schedule: (row tile m, column tile n) of the i-th tile of CTA `cta` of `grid` (`rank`: its rank in a cluster);
+// false when the CTA is out of work.  The producer, the consumers and the host's plan description all enumerate tiles
+// through this one function.
+__host__ __device__ inline bool gemm_tile_index(const GemmGeom& g, int cta, int grid, int rank, int i, int* m, int* n) {
   const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
-  int m, n;
   if (g.sched == 0) {
-    const int t = static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x);
+    const int t = cta + i * grid;
     if (t >= m_tiles * g.n_tiles) return false;
-    n = t % g.n_tiles;
-    m = t / g.n_tiles;
+    *n = t % g.n_tiles;
+    *m = t / g.n_tiles;
   } else if (g.cl_m * g.cl_n == 1) {
-    m = static_cast<int>(blockIdx.x) + (i / g.n_tiles) * static_cast<int>(gridDim.x);
-    if (m >= m_tiles) return false;
-    n = i % g.n_tiles;
+    *m = cta + (i / g.n_tiles) * grid;
+    if (*m >= m_tiles) return false;
+    *n = i % g.n_tiles;
   } else {
     // clusters walk (row super tile, column super tile) in lock step; tiles past the edge ("ghosts") are still processed
     // (zero-filled loads, masked stores) so that every CTA of the cluster performs the same number of pipeline steps
     const int csize = g.cl_m * g.cl_n;
-    const int rank = static_cast<int>(ptx::cluster_ctarank());
     const int n_super = (g.n_tiles + g.cl_n - 1) / g.cl_n;
     const int m_super = (m_tiles + g.cl_m - 1) / g.cl_m;
-    const int ms = static_cast<int>(blockIdx.x) / csize + (i / n_super) * (static_cast<int>(gridDim.x) / csize);
+    const int ms = cta / csize + (i / n_super) * (grid / csize);
     if (ms >= m_super) return false;
-    m = ms * g.cl_m + rank / g.cl_n;
-    n = (i % n_super) * g.cl_n + rank % g.cl_n;
+    *m = ms * g.cl_m + rank / g.cl_n;
+    *n = (i % n_super) * g.cl_n + rank % g.cl_n;
   }
+  return true;
+}
+
+// number of tiles CTA `cta` of `grid` processes
+__host__ inline int gemm_cta_tiles(const GemmGeom& g, int cta, int grid) {
+  int i = 0, m, n;
+  while (gemm_tile_index(g, cta, grid, cta % (g.cl_m * g.cl_n), i, &m, &n)) ++i;
+  return i;
+}
+
+// i-th tile of this CTA under the geometry's schedule; false when the CTA is out of work
+__device__ __forceinline__ bool tile_at(const GemmGeom& g, int i, TileCoord* tc) {
+  const int rank = g.sched != 0 && g.cl_m * g.cl_n > 1 ? static_cast<int>(ptx::cluster_ctarank()) : 0;
+  int m, n;
+  if (!gemm_tile_index(g, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x), rank, i, &m, &n)) return false;
   *tc = decode_tile(g, m, n);
   return true;
 }
@@ -427,6 +447,98 @@ __device__ __forceinline__ void gemm_consumer(const GemmMaps& maps, const GemmGe
   if (lane == 0) ptx::bulk_wait_read0();         // staging tile must outlive the last TMA store's read
 }
 
+// Ping-pong consumer warpgroup wg (GemmGeom::pingpong): tiles wg, wg + 2, ... of this CTA's sequence, each 128 rows x 64
+// columns -- per k16 step and product one m64n64k16 per row half (acc*[0]: tile rows 0..63, acc*[1]: 64..127), so every
+// output element sees the products, accumulator classes and k order of the cooperative path.  A ring slot holds one
+// k-block of one tile and has this one reader (empty_bar counts 1 arrival).  Order barrier: turn_bar[w] completes one
+// phase per hand-over to warpgroup w.  A warpgroup waits for its turn before the first wgmma of a tile (tile 0 needs
+// none) and hands over right after committing the tile's last k-block, so slots are read in the producer's order and an
+// mbarrier wait never meets a phase two laps old; it then drains its groups, releases its last slot and runs the
+// epilogue while the other warpgroup's main loop runs.  A warpgroup without a tile never waits, and the last hand-over
+// of a CTA is never waited for.
+template <class Epi>
+__device__ __forceinline__ void gemm_consumer_pingpong(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep,
+                                                       uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                                       uint64_t* turn_bar, uint8_t* stage_out, int wg, int wl, int lane) {
+  constexpr int BN = 64;
+  const int stage_bytes = gemm_stage_bytes(g);
+  const int nkb = g.R * g.S * g.cin_blocks + g.res_kb;
+  const int num_kb = g.R * g.S * g.cin_blocks;
+  const bool signaller = wl == 0 && lane == 0;
+  float acc0[2][BN / 2], acc1[2][BN / 2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc0[h][i] = acc1[h][i] = 0.f;
+  FragCtx f;
+  f.g = &g;
+  f.maps = &maps;
+  f.lane = lane;
+  f.stage = stage_out;
+  f.store_seq = 0;
+  TileCoord tc;
+  for (int ti = wg; tile_at(g, ti, &tc); ti += 2) {
+    const int pos = ti * nkb;                    // ring position of the tile's first k-block (every tile has nkb)
+    int stage = pos % g.stages;
+    uint32_t phase = static_cast<uint32_t>(pos / g.stages) & 1u;
+    if (ti > 0) ptx::mbar_wait(&turn_bar[wg], static_cast<uint32_t>((ti - 1) >> 1) & 1u);
+    uint32_t started = 0;
+    int pend = -1;
+    for (int kb = 0; kb < nkb; ++kb) {
+      ptx::mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
+      const uint32_t sb = sa + g.nA * kTileABytes;
+      const bool res_block = kb >= num_kb && g.res_kind == 0;
+      const int n_prod = res_block ? g.n_mma_res : g.n_mma;
+      ptx::wgmma_fence();
+      for (int i = 0; i < n_prod; ++i) {
+        const int pa = res_block ? g.mma_res_a[i] : g.mma_a[i];
+        const int pb = res_block ? 0 : g.mma_b[i];
+        const uint64_t bdesc = ptx::make_kmajor_sw128_desc(sb + pb * BN * kBlockK * 2);
+        const uint32_t a_id = static_cast<uint32_t>(res_block ? g.mma_res_acc[i] : g.mma_acc[i]);
+        const uint32_t first = (started >> a_id) & 1u;
+        started |= 1u << a_id;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t adesc = ptx::make_kmajor_sw128_desc(sa + pa * kTileABytes + h * 64 * kBlockK * 2);
+          if (a_id) gemm_mma_kblock<BN, Epi::kBf16>(acc1[h], adesc, bdesc, first);
+          else gemm_mma_kblock<BN, Epi::kBf16>(acc0[h], adesc, bdesc, first);
+        }
+      }
+      ptx::wgmma_commit();
+      if (kb == nkb - 1 && signaller) ptx::mbar_arrive(&turn_bar[wg ^ 1]);   // hand over: every k-block is issued
+      ptx::wgmma_wait<1>();                      // the previous k-block's group is complete: its slot may be refilled
+      if (pend >= 0 && signaller) ptx::mbar_arrive(&empty_bar[pend]);
+      pend = stage;
+      if (++stage == g.stages) { stage = 0; phase ^= 1u; }
+    }
+    ptx::wgmma_wait<0>();
+    if (signaller) ptx::mbar_arrive(&empty_bar[pend]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      ptx::reg_fence(acc0[h]);
+      ptx::reg_fence(acc1[h]);
+    }
+    f.col0 = tc.n_tile * BN;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row0 = h * 64 + wl * 16;                      // this warp's 16 tile rows of row half h
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = row0 + (lane >> 2) + 8 * hr;
+        const int n = tc.n0 + r / (g.tw * g.th), hh = tc.h0 + (r / g.tw) % g.th, w = tc.w0 + r % g.tw;
+        f.valid[hr] = n < g.Nimg && hh < g.Ho && w < g.Wo;
+        f.pix[hr] = (static_cast<long long>(n) * g.Ho + hh) * g.Wo + w;
+      }
+      f.bw0 = tc.w0 + row0 % g.tw;
+      f.bh0 = tc.h0 + (row0 / g.tw) % g.th;
+      f.bn0 = tc.n0 + row0 / (g.tw * g.th);
+      Epi::template run_frag<BN>(ep, f, acc0[h], acc1[h], g.n_acc == 2);
+    }
+  }
+  if (lane == 0) ptx::bulk_wait_read0();         // staging tile must outlive the last TMA store's read
+}
+
 template <class Epi>
 // 12 warps = 3 warpgroups -> 168 registers per thread at launch, redistributed by role (kProducerRegs / kConsumerRegs)
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -447,6 +559,7 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
   uint64_t* empty_bar = bars + g.stages;         // [stages]
   uint64_t* bfull_bar = bars + 2 * g.stages;     // [stages_b]   (halo mode)
   uint64_t* bempty_bar = bfull_bar + 8;          // [stages_b]
+  uint64_t* turn_bar = bempty_bar + 8;           // [2]          (ping-pong order barrier)
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // provably warp-uniform for the compiler
   const int lane = threadIdx.x & 31;
@@ -461,9 +574,12 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
     const int n_peers = g.cl_m + g.cl_n - 1;       // CTAs that read what I multicast == CTAs that multicast to me
     for (int s = 0; s < g.stages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 2 * (g.halo ? 1 : n_peers));   // both consumer warpgroups of every CTA that reads my
-                                                                    // slices (halo patches are never shared)
+      ptx::mbar_init(&empty_bar[s], g.pingpong ? 1 : 2 * (g.halo ? 1 : n_peers));   // ping-pong: the tile's warpgroup;
+                                      // else both consumer warpgroups of every CTA that reads my slices (halo patches are
+                                      // never shared)
     }
+    ptx::mbar_init(&turn_bar[0], 1);
+    ptx::mbar_init(&turn_bar[1], 1);
     if (g.halo)
       for (int s = 0; s < g.stages_b; ++s) {
         ptx::mbar_init(&bfull_bar[s], 1);
@@ -631,7 +747,14 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
     c.extra = extra_smem;
     c.prev_m_tile = -1;
     c.store_seq = 0;
-    switch (g.block_n) {
+    bool done = false;
+    if constexpr (Epi::kFragment) {
+      if (g.pingpong) {
+        gemm_consumer_pingpong<Epi>(maps, g, ep, smem, full_bar, empty_bar, turn_bar, c.stage, wg, wl, lane);
+        done = true;
+      }
+    }
+    if (!done) switch (g.block_n) {
       case 64:
         gemm_consumer<Epi, 64>(maps, g, ep, smem, smem_b, acc_smem, full_bar, empty_bar, bfull_bar, bempty_bar, c, wg, wl,
                                mask_peers, mask_b, csize);

@@ -56,6 +56,8 @@ for _ in range(a.reps):
     enc.profile_read()
 enc.set_profile(False)
 gpu_after = card()
+# ping-pong consumers per layer (tile_gemm.cuh); builds without them do not report the field
+pingpong = {s["layer"]: s.get("pingpong", 0) for s in enc.describe_plan()["steps"] if s["kind"] == "conv"}
 rows = []
 for i, r in enumerate(runs[0]):
     r = dict(r)
@@ -66,9 +68,9 @@ lines = [f"# encoder tile-engine launches, batch {a.batch}, precision {a.precisi
          f"(median of {a.reps} forwards, CUDA events around each launch, so launch gaps are excluded)", "",
          f"GPU (name, power limit, SM clock, max SM clock) before / after the timed forwards: {gpu_before} / {gpu_after}", "",
          f"roofline denominators ({pk['source']}): HBM {hbm:.0f} GB/s, 16-bit dense {tens:.0f} TFLOP/s; "
-         "`frac` = max(bytes/HBM, executed flops/tensor) / time", "",
-         "| layer | M | K | N | bn | kblk | tiles | stg | us | useful TF/s | exec TF/s | GB/s | t_hbm us | t_mma us | frac |",
-         "|---|---|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
+         "`frac` = max(bytes/HBM, executed flops/tensor) / time; `pp` = 1 for ping-pong launches", "",
+         "| layer | M | K | N | bn | kblk | tiles | stg | us | useful TF/s | exec TF/s | GB/s | t_hbm us | t_mma us | frac | pp |",
+         "|---|---|---|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
 for r in rows:
     us = r["ms"] * 1e3
     ex = r["flops"] * r["products"]
@@ -76,7 +78,7 @@ for r in rows:
     t_m = ex / (tens * 1e12) * 1e6
     lines.append(f"| {r['name']} | {r['M']} | {r['K']} | {r['N']} | {r['block_n']} | {r['k_blocks']} | {r['tiles']} | {r['stages']} | {us:.1f} | "
                  f"{r['flops'] / us / 1e6:.0f} | {ex / us / 1e6:.0f} | {r['bytes'] / us / 1e3:.0f} | {t_h:.1f} | {t_m:.1f} | "
-                 f"{max(t_h, t_m) / us:.2f} |")
+                 f"{max(t_h, t_m) / us:.2f} | {pingpong.get(r['name'], 0)} |")
 ideal = sum(max(r["bytes"] / (hbm * 1e9), r["flops"] * r["products"] / (tens * 1e12)) for r in rows) * 1e6
 lines += ["", f"sum of per-layer roofline times: {ideal:.0f} us = {ideal / (tot * 1e3):.2f} of the measured {tot * 1e3:.0f} us"]
 txt = "\n".join(lines) + "\n"
