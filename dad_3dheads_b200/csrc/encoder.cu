@@ -116,9 +116,6 @@ struct dad3d_encoder {
   int num_sms = 0;
   int P = 3;                       // pieces per operand
   int fp16 = 0;                    // piece format: 0 = bf16 (1-3 pieces), 1 = fp16 hi/lo (per-channel scaled weights)
-  int n_mma = 6;
-  int n_acc = 2;
-  int mma_a[kMaxMma], mma_b[kMaxMma], mma_acc[kMaxMma];
   std::map<std::string, ConvW> convs;
   float* d_stem_w = nullptr;       // [147][64]
   float* d_stem_b = nullptr;       // [64]
@@ -128,7 +125,8 @@ struct dad3d_encoder {
   bool stem_simt = false;          // env DAD3D_STEM_SIMT=1: run the stem on the fp32 CUDA-core kernel instead of the tile engine
   bool use_halo = true;            // halo-reuse tiles for the 3x3 stride-1 layers (env DAD3D_HALO=0 selects the per-tap path)
   int halo_cluster = 1;            // env DAD3D_HALO_CLUSTER=2: halo layers run as clusters of 2 row tiles that multicast the weights
-  bool kernels_configured = false, stem_configured = false;   // cudaFuncSetAttribute done on this handle's device
+  GemmLaunchCache gemm_cache;      // the tile engine of this handle's operand format (the only one it launches)
+  bool stem_configured = false;    // cudaFuncSetAttribute done on this handle's device
   bool td_parity = false;          // env DAD3D_TD_PARITY=1: large top-down nodes as four parity launches
   bool heat_sparse = true;         // env DAD3D_HEAT_SPARSE=0: always compute the full heat-map
   bool use_pdl = false;            // programmatic dependent launch for the tile-engine kernels (env DAD3D_PDL=1 enables)
@@ -508,6 +506,7 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     if (s.stem) { g.cin_blocks = 1; g.pad_h = 2; g.pad_w = 0; }   // 4 vertical taps x one 64-element window
     if (s.parity) { g.pad_h = -((s.parity - 1) >> 1); g.pad_w = -((s.parity - 1) & 1); }   // input pixel (2i + a, 2j + b)
     g.cl_m = 1; g.cl_n = 1;
+    gemm_products(g, enc->P);
     const bool res_in_k = s.res >= 0 && s.res_mode == 1 && w->has_identity;
     // few row tiles (small maps / small batch): halve the tile width so that twice as many CTAs share the work
     const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
@@ -525,20 +524,16 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
     const int kb64 = w->R * w->S * g.cin_blocks + (res_in_k ? 1 : src2 ? cin2 / kBlockK : 0);   // k-blocks at block_n 64
     fit.block_n = 64;
     g.pingpong = g.frag_epi && !halo && (w->block_n == 64 || w->has_b64) && gemm_max_stages(fit) >= 2 &&
-                 enc->n_mma > 1 && kb64 <= kPingPongMaxKb ? 1 : 0;
+                 g.n_mma > 1 && kb64 <= kPingPongMaxKb ? 1 : 0;
     const int block_n = narrow || g.pingpong ? 64 : w->block_n;
     g.block_n = block_n;
     g.n_tiles = w->cout_pad / block_n;
-    g.nA = enc->P; g.nB = enc->P;
-    g.n_mma = enc->n_mma;
-    g.n_acc = enc->n_acc;
-    for (int i = 0; i < enc->n_mma; ++i) { g.mma_a[i] = enc->mma_a[i]; g.mma_b[i] = enc->mma_b[i]; g.mma_acc[i] = enc->mma_acc[i]; }
     if (res_in_k) {                                   // "+ identity(x)" performed by the tensor core
       g.res_kb = block_n / kBlockK;
       g.n_mma_res = enc->P;
       for (int i = 0; i < enc->P; ++i) {
         g.mma_res_a[i] = enc->P - 1 - i;              // smallest piece first
-        g.mma_res_acc[i] = (enc->n_acc == 2 && g.mma_res_a[i] != 0) ? 1 : 0;
+        g.mma_res_acc[i] = (g.n_acc == 2 && g.mma_res_a[i] != 0) ? 1 : 0;
       }
     }
     if (src2) {                                       // projection shortcut as a second K segment
@@ -664,23 +659,7 @@ double conv_useful_flops(const Step& s) {
   return 2.0 * g.Nimg * rows * g.Wo * cout * cin * w->R * w->S;
 }
 
-// CTAs of a conv launch: one per SM at most, a whole number of clusters
-int conv_grid(const dad3d_encoder* enc, const GemmGeom& g) {
-  const int m_tiles_total = g.tiles_w * g.tiles_h * g.tiles_n;
-  const int csz = g.cl_m * g.cl_n;
-  if (csz > 1) return std::min(((m_tiles_total + g.cl_m - 1) / g.cl_m) * csz, (enc->num_sms / csz) * csz);
-  return std::min(m_tiles_total * g.n_tiles, enc->num_sms);
-}
-
 int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
-  if (!enc->kernels_configured) {                  // function attributes are per device: remembered per handle
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConv>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<EpiConvH>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
-    enc->kernels_configured = true;
-  }
-  const GemmGeom& g = s.geom;
-  const int grid = conv_grid(enc, g);
-  const int csz = g.cl_m * g.cl_n;
   std::pair<cudaEvent_t, cudaEvent_t>* ev = nullptr;
   if (enc->profile) {
     if (enc->prof_used == enc->prof_events.size()) {
@@ -695,34 +674,11 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
     enc->prof_flops += conv_useful_flops(s);
     DAD3D_CUDA_OK(cudaEventRecord(ev->first, stream));
   }
-  {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = gemm_smem_bytes(g);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (enc->use_pdl) {
-      attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[na].val.programmaticStreamSerializationAllowed = 1;
-      ++na;
-    }
-    if (csz > 1) {
-      attr[na].id = cudaLaunchAttributeClusterDimension;
-      attr[na].val.clusterDim.x = static_cast<unsigned>(csz);
-      attr[na].val.clusterDim.y = 1;
-      attr[na].val.clusterDim.z = 1;
-      ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    if (enc->fp16) DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConvH>, s.maps, g, s.epi));
-    else DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<EpiConv>, s.maps, g, s.epi));
-  }
-  count_launch();
+  const int rc = enc->fp16
+                     ? gemm_launch<EpiConvH>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->use_pdl, stream)
+                     : gemm_launch<EpiConv>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->use_pdl, stream);
+  if (rc != DAD3D_OK) return rc;
   if (ev) DAD3D_CUDA_OK(cudaEventRecord(ev->second, stream));
-  DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
 }
 
@@ -853,18 +809,6 @@ int dad3d_encoder_create(dad3d_encoder** out, const dad3d_conv_weights* layers, 
   enc->num_sms = prop.multiProcessorCount;
   enc->P = pieces;
   enc->fp16 = operand_format == DAD3D_OPERAND_FP16 ? 1 : 0;
-  // product list, smallest terms first so they are not swamped in the fp32 accumulator
-  if (pieces == 1) {
-    enc->n_mma = 1; enc->n_acc = 1; enc->mma_a[0] = 0; enc->mma_b[0] = 0; enc->mma_acc[0] = 0;
-  } else if (pieces == 2) {
-    const int pa[3] = {1, 0, 0}, pb[3] = {0, 1, 0}, pc[3] = {1, 1, 0};
-    enc->n_mma = 3; enc->n_acc = 2;
-    for (int i = 0; i < 3; ++i) { enc->mma_a[i] = pa[i]; enc->mma_b[i] = pb[i]; enc->mma_acc[i] = pc[i]; }
-  } else {
-    const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0}, pc[6] = {1, 1, 1, 1, 1, 0};
-    enc->n_mma = 6; enc->n_acc = 2;
-    for (int i = 0; i < 6; ++i) { enc->mma_a[i] = pa[i]; enc->mma_b[i] = pb[i]; enc->mma_acc[i] = pc[i]; }
-  }
   std::memcpy(enc->bifpn_w, bifpn_fusion_w_h, sizeof(enc->bifpn_w));
   {
     const char* e = std::getenv("DAD3D_PDL");
@@ -1196,7 +1140,12 @@ int dad3d_encoder_describe_plan(dad3d_encoder* enc, char* buf, size_t cap) {
       num("frag_epi", g.frag_epi); num("res_kb", g.res_kb); num("res_kind", g.res_kind); num("res_stride", g.res_stride);
       num("up2", s.up2); num("parity", s.parity); num("rowmap_n", g.rowmap_n); num("n_mma", g.n_mma); num("n_acc", g.n_acc);
       num("cout", s.w->cout); num("cin", s.w->cin); num("has_identity", s.w->has_identity ? 1 : 0);
-      const int grid = conv_grid(enc, g);
+      cudaLaunchConfig_t cfg;
+      cudaLaunchAttribute attr[2];
+      const int rc = enc->fp16 ? gemm_launch_config<EpiConvH>(g, enc->num_sms, &enc->gemm_cache, enc->use_pdl, &cfg, attr)
+                               : gemm_launch_config<EpiConv>(g, enc->num_sms, &enc->gemm_cache, enc->use_pdl, &cfg, attr);
+      if (rc != DAD3D_OK) return rc;
+      const int grid = static_cast<int>(cfg.gridDim.x);
       int tmin = 1 << 30, tmax = 0;
       for (int b = 0; b < grid; ++b) {
         const int t = gemm_cta_tiles(g, b, grid);

@@ -130,7 +130,6 @@ struct EpiConvParams {
 
 template <bool F16>
 struct EpiConvT {
-  static constexpr int kExtraSmemBytes = 0;
   static constexpr int kBf16 = F16 ? 0 : 1;       // operand format of the tile engine
   static constexpr bool kFragment = true;         // piece outputs (ep.out != nullptr) run on the register fragments
   struct State {};

@@ -1,9 +1,17 @@
-// FLAME head decoder for sm_90a:  413 params -> 5023x3 vertices (+ weak-perspective projection) in three kernels
-//   K1 flame_prep_kernel    per-head small math: betas -> fp16 hi/lo coefficient rows, folded joint regression,
-//                           Rodrigues, kinematic chain, 6-DoF rotation folded into the skinning transforms
-//   K2 tile_gemm_kernel<EpiBlend>   blend shapes + pose correctives as ONE wgmma GEMM  [heads,448] x [15069,448]^T
+// FLAME head decoder for sm_90a:  413 params -> 5023x3 vertices (+ weak-perspective projection), and its backward.
+// Every pass starts with K1, flame_prep_kernel: per-head small math (betas -> fp16 hi/lo coefficient rows, folded joint
+// regression, Rodrigues, kinematic chain, 6-DoF rotation folded into the skinning transforms).  The blend product
+// [heads,448] x [15069,448]^T (blend shapes + pose correctives + template) and the skinning then take one of four paths,
+// chosen by decode_path:
+//   dedicated  (default, layouts with only the jaw posed) flame_decode_kernel (flame_decode.cuh): one fp16 product per MAC,
+//              skinning, z offset, rotation and projection in its epilogue
+//   lbs        (DAD3D_BLEND_HILO) K2 tile_gemm_kernel<EpiLbs>: fp16 hi/lo operands, 3 products (fp32-class), the same
+//              skinning in the epilogue; with DAD3D_DECODE_CLUSTER big passes run as 2x2 clusters with TMA multicast
+//   blend      (other layouts, DAD3D_DECODE_UNFUSED) K2 tile_gemm_kernel<EpiBlend> to a v_posed scratch, then K3
+//   simt       (DAD3D_BLEND_SIMT) blend_simt_kernel, CUDA-core fp32 product, to the same scratch, then K3
 //   K3 lbs_project_kernel   linear-blend skinning + z offset + rotation + projection, shared-memory staged, coalesced
 //   K4 gather kernels       landmark subsets
+// The backward recomputes the blend product and runs the transposed one on the tile engine (<EpiBlend>, hi/lo operands).
 // Reference math: model_training/model/flame.py:182-229, smplx.lbs (0.1.26), model_training/model/utils.py:92-101,
 // model_training/head_mesh.py:33-46.  See DESIGN.md for layouts and rooflines.
 #include <cuda_fp16.h>
@@ -213,7 +221,6 @@ flame_prep_kernel(const float* __restrict__ params, int B, FlameLayoutDev L, con
 
 // ------------------------------------------------------------------------------------------------ K2 epilogue
 struct EpiBlend {
-  static constexpr int kExtraSmemBytes = 0;
   static constexpr int kBf16 = 0;                 // fp16 operands
   static constexpr bool kFragment = false;        // row epilogue over the shared-memory accumulator tile
   struct State {};
@@ -245,7 +252,6 @@ struct EpiBlend {
 // 16*grp.. of the tile, as two passes of 8 vertices (24 accumulator columns).  Results are staged per warp so that global
 // stores are contiguous runs (the reference layout's 60 276-byte row pitch rules out TMA stores).
 struct EpiLbs {
-  static constexpr int kExtraSmemBytes = 0;
   static constexpr int kBf16 = 0;                 // fp16 operands
   static constexpr bool kFragment = false;        // row epilogue over the shared-memory accumulator tile
   struct Params {
@@ -783,9 +789,8 @@ using namespace dad3d;
 
 struct dad3d_flame {
   int device = 0;
-  int smem_configured[3] = {0, 0, 0};        // per handle (= per device): max dynamic smem set for <EpiLbs> / <EpiBlend> /
-                                             // flame_decode_kernel
-  int max_clusters[1] = {0};                 // per handle: co-resident 2x2 tile-engine clusters
+  GemmLaunchCache gemm_lbs, gemm_blend;      // tile-engine launches with <EpiLbs> / <EpiBlend>
+  bool decode_configured = false;            // per handle (= per device): max dynamic smem set for flame_decode_kernel
   int nv = 0, n3 = 0, npad = 0;
   int num_sms = 0;
   FlameLayoutDev layout{};
@@ -810,59 +815,6 @@ struct dad3d_flame {
 
 namespace {
 
-// Launch configuration of one tile-engine launch: grid size (CTAs) in *grid.  Shared by the launch and dad3d_flame_describe.
-template <class Epi>
-int tile_gemm_config(const GemmGeom& g, int num_sms, int* configured, int* max_clusters_cache, cudaLaunchConfig_t* cfg,
-                     cudaLaunchAttribute* attr) {
-  // function attributes are per device: remembered in the handle, not in a process-wide static
-  const int smem = gemm_smem_bytes(g, Epi::kExtraSmemBytes);
-  if (!*configured) {
-    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
-    *configured = 1;
-  }
-  const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
-  const int csize = g.cl_m * g.cl_n;
-  *cfg = cudaLaunchConfig_t{};
-  cfg->blockDim = dim3(kGemmThreads);
-  cfg->dynamicSmemBytes = smem;
-  cfg->attrs = attr;
-  cfg->numAttrs = 0;
-  if (csize > 1) {
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = csize;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg->numAttrs = 1;
-    int& max_clusters = *max_clusters_cache;           // co-resident clusters of this size (GPC packing: < #SM / csize);
-    if (max_clusters == 0) {                           // cached in the handle: occupancy is a per-device property
-      cfg->gridDim = dim3(num_sms / csize * csize);
-      DAD3D_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, tile_gemm_kernel<Epi>, cfg));
-      if (max_clusters < 1) { set_error("no co-resident cluster fits"); return DAD3D_ERR_CUDA; }
-    }
-    const int m_super = ceil_div(m_tiles, g.cl_m);
-    const int clusters = m_super < max_clusters ? m_super : max_clusters;
-    cfg->gridDim = dim3(clusters * csize);
-  } else {
-    const int total = g.sched == 1 ? m_tiles : m_tiles * g.n_tiles;
-    cfg->gridDim = dim3(total < num_sms ? total : num_sms);
-  }
-  return DAD3D_OK;
-}
-
-template <class Epi>
-int launch_tile_gemm(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep, int num_sms,
-                     cudaStream_t stream, int* configured, int* max_clusters_cache) {
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  const int rc = tile_gemm_config<Epi>(g, num_sms, configured, max_clusters_cache, &cfg, attr);
-  if (rc != DAD3D_OK) return rc;
-  cfg.stream = stream;
-  DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<Epi>, maps, g, ep));
-  count_launch();
-  DAD3D_CUDA_OK(cudaGetLastError());
-  return DAD3D_OK;
-}
-
 // Schedule of one flame_decode_kernel launch over `rows` heads: fills rows, nv, n_tiles, m_units, splits and stages of *p and
 // returns the grid size (CTAs).  Shared by the launch and dad3d_flame_describe.
 int dec_schedule(const dad3d_flame* h, int rows, DecodeParams* p) {
@@ -883,10 +835,10 @@ int dec_schedule(const dad3d_flame* h, int rows, DecodeParams* p) {
 // kernel has written.
 int launch_flame_decode(dad3d_flame* h, const __half* a_hi, int rows, const float* xf, float* v3, float* pj, int pc,
                         float image_size, cudaStream_t stream) {
-  if (!h->smem_configured[2]) {
+  if (!h->decode_configured) {
     DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
     DAD3D_CUDA_OK(cudaFuncSetAttribute(flame_decode_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemLimit));
-    h->smem_configured[2] = 1;
+    h->decode_configured = true;
   }
   CUtensorMap map_a;
   {
@@ -1174,37 +1126,47 @@ static bool decode_clustered(const dad3d_flame* h, DecodePath path, int rows, in
   return path == kPathLbs && ceil_div(rows, kBlockM) >= h->num_sms && (flags & DAD3D_DECODE_CLUSTER);
 }
 
-// Tile-engine geometry of the blend product of one pass (kPathLbs / kPathBlend)
-static GemmGeom blend_geom(const dad3d_flame* h, DecodePath path, int rows, int flags) {
-  const bool fused = path == kPathLbs;
-  const bool clustered = decode_clustered(h, path, rows, flags);
-  const int block_n = fused ? kFusedBlockN : kBlendBlockN;
+// Tile-engine geometry of a plain row GEMM  D[rows, n_cols] = A[rows, 64 k_blocks] B[n_cols, 64 k_blocks]^T  with
+// `pieces`-piece operands: single CTAs, tiles round-robin, the deepest operand ring that fits
+static GemmGeom row_gemm_geom(int rows, int k_blocks, int n_cols, int block_n, int pieces) {
   GemmGeom g;
   std::memset(&g, 0, sizeof(g));
   g.tw = kBlockM; g.th = 1; g.tn = 1;
   g.tiles_w = ceil_div(rows, kBlockM); g.tiles_h = 1; g.tiles_n = 1;
   g.Wo = rows; g.Ho = 1; g.Nimg = 1;
-  g.stride = 1; g.R = 1; g.S = 1; g.pad_h = 0; g.pad_w = 0;
-  g.cin_blocks = kKPad / kBlockK;
-  g.cl_m = clustered ? 2 : 1;
-  g.cl_n = clustered ? 2 : 1;
-  g.n_tiles = ceil_div(h->n3, block_n);
+  g.stride = 1; g.R = 1; g.S = 1;
+  g.cin_blocks = k_blocks;
+  g.cl_m = 1; g.cl_n = 1;
+  g.n_tiles = ceil_div(n_cols, block_n);
   g.block_n = block_n;
-  if ((flags & DAD3D_BLEND_FAST) && !(flags & DAD3D_BLEND_HILO)) {      // unfused A/B path with one product
-    g.nA = 1; g.nB = 1; g.n_mma = 1; g.mma_a[0] = 0; g.mma_b[0] = 0; g.mma_acc[0] = 0; g.n_acc = 1;
-  } else {
-    g.nA = 2; g.nB = 2; g.n_mma = 3; g.n_acc = 2;
-    g.mma_a[0] = 1; g.mma_b[0] = 0; g.mma_acc[0] = 1;   // lo*hi, hi*lo: small terms, own accumulator
-    g.mma_a[1] = 0; g.mma_b[1] = 1; g.mma_acc[1] = 1;
-    g.mma_a[2] = 0; g.mma_b[2] = 0; g.mma_acc[2] = 0;   // hi*hi
+  gemm_products(g, pieces);
+  g.stages = gemm_max_stages(g);
+  return g;
+}
+
+// Tensor maps of a row GEMM: A = the fp16 plane pair hi / lo, each [rows, k] (box 64 x box_rows), and the B planes b[0..1]
+static int row_gemm_maps(GemmMaps* maps, const __half* hi, const __half* lo, int rows, int k, int box_rows,
+                         const CUtensorMap* b) {
+  std::memset(maps, 0, sizeof(*maps));
+  const __half* planes[2] = {hi, lo};
+  for (int pi = 0; pi < 2; ++pi) {
+    const uint64_t dims[4] = {static_cast<uint64_t>(k), static_cast<uint64_t>(rows), 1, 1};
+    const uint64_t strides[3] = {static_cast<uint64_t>(k) * 2, static_cast<uint64_t>(k) * 2 * rows,
+                                 static_cast<uint64_t>(k) * 2 * rows};
+    const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(box_rows), 1, 1};
+    if (!make_tmap_16bit(&maps->a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
+    maps->b[pi] = b[pi];
   }
-  if (fused) {
-    g.sched = g.tiles_w >= h->num_sms ? 1 : 0;          // enough row tiles to give every SM its own
-    g.stages = gemm_max_stages(g, EpiLbs::kExtraSmemBytes);
-  } else {
-    g.sched = 0;
-    g.stages = gemm_max_stages(g);
-  }
+  return DAD3D_OK;
+}
+
+// Tile-engine geometry of the blend product of one pass (kPathLbs / kPathBlend)
+static GemmGeom blend_geom(const dad3d_flame* h, DecodePath path, int rows, int flags) {
+  const bool fused = path == kPathLbs;
+  const int pieces = (flags & DAD3D_BLEND_FAST) && !(flags & DAD3D_BLEND_HILO) ? 1 : 2;   // unfused A/B path: one product
+  GemmGeom g = row_gemm_geom(rows, kKPad / kBlockK, h->n3, fused ? kFusedBlockN : kBlendBlockN, pieces);
+  if (decode_clustered(h, path, rows, flags)) { g.cl_m = 2; g.cl_n = 2; }
+  g.sched = fused && g.tiles_w >= h->num_sms ? 1 : 0;   // enough row tiles to give every SM its own
   return g;
 }
 
@@ -1234,23 +1196,16 @@ static int flame_decode_stage(dad3d_flame* h, const __half* a_hi, const __half* 
   } else {
     const bool clustered = decode_clustered(h, path, rows, flags);
     GemmMaps maps;
-    std::memset(&maps, 0, sizeof(maps));
-    const __half* planes[2] = {a_hi, a_lo};
-    for (int pi = 0; pi < 2; ++pi) {
-      const uint64_t dims[4] = {static_cast<uint64_t>(kKPad), static_cast<uint64_t>(rows), 1, 1};
-      const uint64_t strides[3] = {static_cast<uint64_t>(kKPad) * 2, static_cast<uint64_t>(kKPad) * 2 * rows,
-                                   static_cast<uint64_t>(kKPad) * 2 * rows};
-      const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(clustered ? kBlockM / 2 : kBlockM), 1, 1};
-      if (!make_tmap_16bit(&maps.a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
-      maps.b[pi] = path == kPathLbs ? (clustered ? h->map_b48[pi] : h->map_b96[pi]) : h->map_b[pi];
-    }
+    int rc = row_gemm_maps(&maps, a_hi, a_lo, rows, kKPad, clustered ? kBlockM / 2 : kBlockM,
+                           path == kPathLbs ? (clustered ? h->map_b48 : h->map_b96) : h->map_b);
+    if (rc != DAD3D_OK) return rc;
     const GemmGeom g = blend_geom(h, path, rows, flags);
     if (path == kPathLbs) {
       EpiLbs::Params ep{xf, h->d_w2, h->nv, v3, pj, pc, image_size};
-      return launch_tile_gemm<EpiLbs>(maps, g, ep, h->num_sms, stream, &h->smem_configured[0], &h->max_clusters[0]);
+      return gemm_launch<EpiLbs>(maps, g, ep, h->num_sms, &h->gemm_lbs, false, stream);
     }
     EpiBlend::Params ep{vposed, h->npad};
-    int rc = launch_tile_gemm<EpiBlend>(maps, g, ep, h->num_sms, stream, &h->smem_configured[1], &h->max_clusters[0]);
+    rc = gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
     if (rc != DAD3D_OK) return rc;
   }
   dim3 grid(ceil_div(h->nv, kLbsThreads), rows < 1024 ? rows : 1024);
@@ -1347,10 +1302,9 @@ int dad3d_flame_describe(dad3d_flame* h, int32_t B, int32_t flags, char* json, s
     } else {
       const GemmGeom g = blend_geom(h, path, rows, flags);
       cudaLaunchConfig_t cfg;
-      cudaLaunchAttribute attr[1];
-      int rc = path == kPathLbs
-                   ? tile_gemm_config<EpiLbs>(g, h->num_sms, &h->smem_configured[0], &h->max_clusters[0], &cfg, attr)
-                   : tile_gemm_config<EpiBlend>(g, h->num_sms, &h->smem_configured[1], &h->max_clusters[0], &cfg, attr);
+      cudaLaunchAttribute attr[2];
+      int rc = path == kPathLbs ? gemm_launch_config<EpiLbs>(g, h->num_sms, &h->gemm_lbs, false, &cfg, attr)
+                                : gemm_launch_config<EpiBlend>(g, h->num_sms, &h->gemm_blend, false, &cfg, attr);
       if (rc != DAD3D_OK) return rc;
       m_units = g.tiles_w;
       grid = static_cast<int>(cfg.gridDim.x);
@@ -1400,13 +1354,6 @@ static int ensure_backward_assets(dad3d_flame* h) {
   return DAD3D_OK;
 }
 
-static void hilo_products(GemmGeom& g) {
-  g.nA = 2; g.nB = 2; g.n_mma = 3; g.n_acc = 2;
-  g.mma_a[0] = 1; g.mma_b[0] = 0; g.mma_acc[0] = 1;
-  g.mma_a[1] = 0; g.mma_b[1] = 1; g.mma_acc[1] = 1;
-  g.mma_a[2] = 0; g.mma_b[2] = 0; g.mma_acc[2] = 0;
-}
-
 int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, const float* grad_vertices_d,
                          const float* grad_projected_d, float image_size, int32_t to_2d, float* grad_params_d,
                          void* workspace_d, size_t workspace_bytes, dad3d_stream stream_) {
@@ -1448,31 +1395,11 @@ int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32
     DAD3D_CUDA_OK(cudaGetLastError());
     {   // forward blend product (recomputed): v_posed * basis_scale -> scratch
       GemmMaps maps;
-      std::memset(&maps, 0, sizeof(maps));
-      __half* planes[2] = {a_hi, a_lo};
-      for (int pi = 0; pi < 2; ++pi) {
-        const uint64_t dims[4] = {static_cast<uint64_t>(kKPad), static_cast<uint64_t>(rows), 1, 1};
-        const uint64_t strides[3] = {static_cast<uint64_t>(kKPad) * 2, static_cast<uint64_t>(kKPad) * 2 * rows,
-                                     static_cast<uint64_t>(kKPad) * 2 * rows};
-        const uint32_t box[4] = {kBlockK, kBlockM, 1, 1};
-        if (!make_tmap_16bit(&maps.a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
-        maps.b[pi] = h->map_b[pi];
-      }
-      GemmGeom g;
-      std::memset(&g, 0, sizeof(g));
-      g.tw = kBlockM; g.th = 1; g.tn = 1;
-      g.tiles_w = ceil_div(rows, kBlockM); g.tiles_h = 1; g.tiles_n = 1;
-      g.Wo = rows; g.Ho = 1; g.Nimg = 1;
-      g.stride = 1; g.R = 1; g.S = 1;
-      g.cin_blocks = kKPad / kBlockK;
-      g.cl_m = 1; g.cl_n = 1;
-      g.block_n = kBlendBlockN;
-      g.n_tiles = ceil_div(h->n3, kBlendBlockN);
-      hilo_products(g);
-      g.sched = 0;
-      g.stages = gemm_max_stages(g);
+      rc = row_gemm_maps(&maps, a_hi, a_lo, rows, kKPad, kBlockM, h->map_b);
+      if (rc != DAD3D_OK) return rc;
+      const GemmGeom g = row_gemm_geom(rows, kKPad / kBlockK, h->n3, kBlendBlockN, 2);
       EpiBlend::Params ep{vposed, h->npad};
-      rc = launch_tile_gemm<EpiBlend>(maps, g, ep, h->num_sms, stream, &h->smem_configured[1], &h->max_clusters[0]);
+      rc = gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
       if (rc != DAD3D_OK) return rc;
     }
     flame_bwd_gmax_kernel<<<rows, 256, 0, stream>>>(gv, gp, pc, h->nv, xf, half_img, sigma);
@@ -1489,31 +1416,11 @@ int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32
     }
     {   // the dense part: d coef [rows, 448] = D [rows, 15104] x Basis_s [15104, 448]   (wgmma, fp16 hi/lo, 3 products)
       GemmMaps maps;
-      std::memset(&maps, 0, sizeof(maps));
-      __half* planes[2] = {d_hi, d_lo};
-      for (int pi = 0; pi < 2; ++pi) {
-        const uint64_t dims[4] = {static_cast<uint64_t>(h->npad), static_cast<uint64_t>(rows), 1, 1};
-        const uint64_t strides[3] = {static_cast<uint64_t>(h->npad) * 2, static_cast<uint64_t>(h->npad) * 2 * rows,
-                                     static_cast<uint64_t>(h->npad) * 2 * rows};
-        const uint32_t box[4] = {kBlockK, kBlockM, 1, 1};
-        if (!make_tmap_16bit(&maps.a[pi], planes[pi], 4, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
-        maps.b[pi] = h->map_bT[pi];
-      }
-      GemmGeom g;
-      std::memset(&g, 0, sizeof(g));
-      g.tw = kBlockM; g.th = 1; g.tn = 1;
-      g.tiles_w = ceil_div(rows, kBlockM); g.tiles_h = 1; g.tiles_n = 1;
-      g.Wo = rows; g.Ho = 1; g.Nimg = 1;
-      g.stride = 1; g.R = 1; g.S = 1;
-      g.cin_blocks = h->npad / kBlockK;
-      g.cl_m = 1; g.cl_n = 1;
-      g.block_n = 64;
-      g.n_tiles = kKPad / 64;
-      hilo_products(g);
-      g.sched = 0;
-      g.stages = gemm_max_stages(g);
+      rc = row_gemm_maps(&maps, d_hi, d_lo, rows, h->npad, kBlockM, h->map_bT);
+      if (rc != DAD3D_OK) return rc;
+      const GemmGeom g = row_gemm_geom(rows, h->npad / kBlockK, kKPad, 64, 2);
       EpiBlend::Params ep{dcoef, kKPad};
-      rc = launch_tile_gemm<EpiBlend>(maps, g, ep, h->num_sms, stream, &h->smem_configured[1], &h->max_clusters[0]);
+      rc = gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
       if (rc != DAD3D_OK) return rc;
     }
     flame_bwd_finalize_kernel<<<ceil_div(rows * 32, 128), 128, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags, inv_scale,

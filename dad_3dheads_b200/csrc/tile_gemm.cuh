@@ -35,7 +35,10 @@
 // taps through shifted descriptors; separate weights ring), res_kb / res_kind (residual or second source on the K axis),
 // cl_m x cl_n multicast clusters, and ping-pong consumers (GemmGeom::pingpong: each warpgroup owns whole 128 x 64 tiles and the
 // two take turns in the main loop, so one warpgroup's epilogue runs under the other's main loop; gemm_consumer_pingpong).
+// Host side (end of file): the product list of a piece count, and the launch configuration and launch of the kernel.
 #pragma once
+#include "../../include/dad3d.h"
+#include "common.h"
 #include "ptx.cuh"
 
 namespace dad3d {
@@ -132,11 +135,11 @@ __host__ __device__ inline int gemm_acc_stride(const GemmGeom& g) { return (g.bl
 __host__ __device__ inline int gemm_acc_bytes(const GemmGeom& g) {
   return g.frag_epi ? 0 : kBlockM * gemm_acc_stride(g) * 4;
 }
-__host__ inline int gemm_fixed_smem_bytes(const GemmGeom& g, int extra = 0) {
-  return kEpiWarps * kStageOutBytes + gemm_acc_bytes(g) + extra + 1024 /*align slack*/ + 512 /*barriers*/;
+__host__ inline int gemm_fixed_smem_bytes(const GemmGeom& g) {
+  return kEpiWarps * kStageOutBytes + gemm_acc_bytes(g) + 1024 /*align slack*/ + 512 /*barriers*/;
 }
-__host__ inline int gemm_max_stages(const GemmGeom& g, int extra = 0) {
-  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(g, extra)) / gemm_stage_bytes(g);
+__host__ inline int gemm_max_stages(const GemmGeom& g) {
+  int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(g)) / gemm_stage_bytes(g);
   return s > 8 ? 8 : s;
 }
 // halo mode: A ring fixed at 2 stages, the rest goes to the weights ring (0 if it does not fit)
@@ -144,9 +147,9 @@ __host__ inline int gemm_halo_b_stages(const GemmGeom& g, int a_stages = 2) {
   int s = (kGemmSmemLimit - gemm_fixed_smem_bytes(g) - a_stages * gemm_halo_a_stage_bytes(g)) / gemm_b_stage_bytes(g);
   return s > 8 ? 8 : s;
 }
-__host__ inline int gemm_smem_bytes(const GemmGeom& g, int extra = 0) {
-  if (g.halo) return g.stages * gemm_halo_a_stage_bytes(g) + g.stages_b * gemm_b_stage_bytes(g) + gemm_fixed_smem_bytes(g, extra);
-  return g.stages * gemm_stage_bytes(g) + gemm_fixed_smem_bytes(g, extra);
+__host__ inline int gemm_smem_bytes(const GemmGeom& g) {
+  if (g.halo) return g.stages * gemm_halo_a_stage_bytes(g) + g.stages_b * gemm_b_stage_bytes(g) + gemm_fixed_smem_bytes(g);
+  return g.stages * gemm_stage_bytes(g) + gemm_fixed_smem_bytes(g);
 }
 
 struct TileCoord {
@@ -222,7 +225,6 @@ struct EpiCtx {
   const float* acc;  // this thread's row of the shared-memory accumulator tile (both accumulator classes summed)
   int swz;           // its 16-byte chunk swizzle (row & 7)
   uint8_t* stage;    // warp-private 4 KiB staging tile (1024-byte aligned)
-  uint8_t* extra;    // Epi::kExtraSmemBytes of CTA-wide shared memory (epilogue-specific use)
   int prev_m_tile;   // row tile of the previous tile this CTA processed (-1 for the first)
   mutable int store_seq;   // number of TMA stores this warp has issued (epilogues alternating between two staging tiles)
   // this thread's accumulator row
@@ -553,8 +555,7 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
   uint8_t* smem_b = smem + g.stages * stage_bytes;                              // [stages_b][nB][block_n x 128 B] (halo mode)
   uint8_t* out_stage = smem_b + (g.halo ? g.stages_b * b_stage_bytes : 0);     // [kEpiWarps][4 KiB]
   float* acc_smem = reinterpret_cast<float*>(out_stage + kEpiWarps * kStageOutBytes);   // [128][gemm_acc_stride]
-  uint8_t* extra_smem = out_stage + kEpiWarps * kStageOutBytes + gemm_acc_bytes(g);     // [Epi::kExtraSmemBytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(extra_smem + Epi::kExtraSmemBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + kEpiWarps * kStageOutBytes + gemm_acc_bytes(g));
   uint64_t* full_bar = bars;                     // [stages]
   uint64_t* empty_bar = bars + g.stages;         // [stages]
   uint64_t* bfull_bar = bars + 2 * g.stages;     // [stages_b]   (halo mode)
@@ -744,7 +745,6 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
     c.acc = acc_smem + row * gemm_acc_stride(g);
     c.swz = row & 7;
     c.stage = out_stage + (warp - kFirstEpiWarp) * kStageOutBytes;
-    c.extra = extra_smem;
     c.prev_m_tile = -1;
     c.store_seq = 0;
     bool done = false;
@@ -776,6 +776,90 @@ tile_gemm_kernel(const __grid_constant__ GemmMaps maps, const GemmGeom g, const 
 
   __syncthreads();
   if (csize > 1) ptx::cluster_sync_all();          // nobody leaves while a peer may still write my smem / barriers
+}
+
+// =================================================================================================== host side
+// Operand pieces and product list of `pieces`-piece operands (1, 2 or 3), smallest terms first so that they are not
+// swamped in the fp32 accumulator; with more than one piece every product but p0*p0 goes to accumulator class 1.
+__host__ inline void gemm_products(GemmGeom& g, int pieces) {
+  static const int pa[3][kMaxMma] = {{0}, {1, 0, 0}, {2, 0, 1, 1, 0, 0}};
+  static const int pb[3][kMaxMma] = {{0}, {0, 1, 0}, {0, 2, 1, 0, 1, 0}};
+  static const int pc[3][kMaxMma] = {{0}, {1, 1, 0}, {1, 1, 1, 1, 1, 0}};
+  g.nA = pieces;
+  g.nB = pieces;
+  g.n_mma = pieces == 1 ? 1 : pieces == 2 ? 3 : 6;
+  g.n_acc = pieces == 1 ? 1 : 2;
+  for (int i = 0; i < g.n_mma; ++i) {
+    g.mma_a[i] = pa[pieces - 1][i];
+    g.mma_b[i] = pb[pieces - 1][i];
+    g.mma_acc[i] = pc[pieces - 1][i];
+  }
+}
+
+// What launches of one tile_gemm_kernel<Epi> remember.  Function attributes and occupancy are per device, so this lives
+// in the handle that owns the launches, not in a process-wide static.
+struct GemmLaunchCache {
+  bool smem_set = false;     // max dynamic shared memory set on the kernel
+  int max_clusters[5] = {};  // co-resident clusters, by cluster size cl_m * cl_n (0: not queried yet)
+};
+
+// Launch configuration of one launch, without the stream: grid, dynamic shared memory, the cluster attribute and, with
+// `pdl`, programmatic dependent launch (`attr` holds two).  At most one CTA per SM: a plain launch runs
+// min(work units, #SM) CTAs, where a work unit is a row tile under sched 1 and a tile otherwise; a clustered launch runs
+// as many whole clusters as are co-resident, at most one per row super tile.
+template <class Epi>
+__host__ int gemm_launch_config(const GemmGeom& g, int num_sms, GemmLaunchCache* cache, bool pdl, cudaLaunchConfig_t* cfg,
+                                cudaLaunchAttribute* attr) {
+  if (!cache->smem_set) {
+    DAD3D_CUDA_OK(cudaFuncSetAttribute(tile_gemm_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemLimit));
+    cache->smem_set = true;
+  }
+  const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
+  const int csize = g.cl_m * g.cl_n;
+  *cfg = cudaLaunchConfig_t{};
+  cfg->blockDim = dim3(kGemmThreads);
+  cfg->dynamicSmemBytes = gemm_smem_bytes(g);
+  cfg->attrs = attr;
+  cfg->numAttrs = 0;
+  if (csize > 1) {
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = csize;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg->numAttrs = 1;
+    int& max_clusters = cache->max_clusters[csize];   // GPC packing: can be fewer than #SM / csize
+    if (max_clusters == 0) {
+      cfg->gridDim = dim3(num_sms / csize * csize);
+      DAD3D_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, tile_gemm_kernel<Epi>, cfg));
+      if (max_clusters < 1) { set_error("no co-resident cluster fits"); return DAD3D_ERR_CUDA; }
+    }
+    const int m_super = ceil_div(m_tiles, g.cl_m);
+    cfg->gridDim = dim3((m_super < max_clusters ? m_super : max_clusters) * csize);
+  } else {
+    const int units = g.sched == 1 ? m_tiles : m_tiles * g.n_tiles;
+    cfg->gridDim = dim3(units < num_sms ? units : num_sms);
+  }
+  if (pdl) {
+    attr[cfg->numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg->numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    ++cfg->numAttrs;
+  }
+  return DAD3D_OK;
+}
+
+// One launch of tile_gemm_kernel<Epi> on `stream`.
+template <class Epi>
+__host__ int gemm_launch(const GemmMaps& maps, const GemmGeom& g, const typename Epi::Params& ep, int num_sms,
+                         GemmLaunchCache* cache, bool pdl, cudaStream_t stream) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[2];
+  const int rc = gemm_launch_config<Epi>(g, num_sms, cache, pdl, &cfg, attr);
+  if (rc != DAD3D_OK) return rc;
+  cfg.stream = stream;
+  DAD3D_CUDA_OK(cudaLaunchKernelEx(&cfg, tile_gemm_kernel<Epi>, maps, g, ep));
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
 }
 
 }  // namespace dad3d
