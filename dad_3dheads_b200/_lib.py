@@ -26,6 +26,13 @@ class FlameLayout(C.Structure):
                                          "scale")]
 
 
+class Lighting(C.Structure):
+    """dad3d_lighting: RenderPipeline's parameters (Sim3DR/lighting.py:24-32), passed by value."""
+    _fields_ = [("intensity_ambient", C.c_float), ("intensity_directional", C.c_float), ("intensity_specular", C.c_float),
+                ("specular_exp", C.c_int32), ("color_ambient", C.c_float * 3), ("color_directional", C.c_float * 3),
+                ("light_pos", C.c_float * 3), ("view_pos", C.c_float * 3)]
+
+
 _lib = None
 
 # every symbol include/dad3d.h declares: (restype, argtypes)
@@ -80,6 +87,11 @@ SIGNATURES = {
                                          C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_vertex_normals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "dad3d_light_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                    Lighting, C.c_void_p, C.c_void_p]),
+    "dad3d_render_lit": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_int32, Lighting, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p]),
     "dad3d_comm_unique_id": (C.c_int, [C.c_void_p]),
     "dad3d_comm_init": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "dad3d_comm_destroy": (None, [C.c_void_p]),

@@ -16,6 +16,8 @@
 //     (pixel, image) and decodes head and triangle from the winner.  Without a map, image = head and the low word is ~triangle.
 //   * vertex normals accumulate the un-normalised face normals of the incident triangles in ascending triangle order (caller-built
 //     CSR adjacency), the order of the reference's scatter loop.
+//   * lit meshes (Sim3DR/lighting.py:23-71 RenderPipeline): light_kernel computes each head's per-vertex light in the
+//     reference's float32 order (the power correctly rounded), and pass 2 takes per-head colour tables (a colour stride).
 // Integer / float HBM-bound work; no tensor cores.
 #include <cstdint>
 
@@ -110,10 +112,11 @@ __global__ void raster_tri_kernel(const float* __restrict__ verts, int nv, int b
 }
 
 // pass 2: one thread per (pixel, image) shades the winning triangle; tri_index gets the winner or -1 in depth-buffer rows.
-// mapped != 0: the key names (head, triangle) as head * ntri + triangle, and head_index gets the head or -1.
+// mapped != 0: the key names (head, triangle) as head * ntri + triangle, and head_index gets the head or -1.  Head b's
+// colours start at colors + b * color_stride (0: every head shares one table).
 __global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, int n_images, const int* __restrict__ tris,
-                                      int ntri, int mapped, const float* __restrict__ colors, int h, int w, int c, int reverse,
-                                      int negate_z, const unsigned long long* __restrict__ key,
+                                      int ntri, int mapped, const float* __restrict__ colors, long long color_stride, int h,
+                                      int w, int c, int reverse, int negate_z, const unsigned long long* __restrict__ key,
                                       unsigned char* __restrict__ image, float* __restrict__ depth, int* __restrict__ tri_index,
                                       int* __restrict__ head_index) {
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
@@ -139,8 +142,9 @@ __global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, i
     if (depth) depth[at] = radd(radd(rmul(wt[0], s.d0), rmul(wt[1], s.d1)), rmul(wt[2], s.d2));
     if (!image) continue;
     unsigned char* px = image + (m * hw + static_cast<long long>(yo) * w + x) * c;
+    const float* col = colors + b * color_stride;                     // the winning head's colours (stride 0: one table)
     for (int ch = 0; ch < c; ++ch) {
-      const float pc = radd(radd(rmul(wt[0], colors[c * s.i0 + ch]), rmul(wt[1], colors[c * s.i1 + ch])), rmul(wt[2], colors[c * s.i2 + ch]));
+      const float pc = radd(radd(rmul(wt[0], col[c * s.i0 + ch]), rmul(wt[1], col[c * s.i1 + ch])), rmul(wt[2], col[c * s.i2 + ch]));
       // (unsigned char)((1 - alpha) * image + alpha * 255 * p_color) with alpha = 1
       const float old = static_cast<float>(px[ch]);
       const float val = radd(rmul(rsub(1.0f, 1.0f), old), rmul(rmul(1.0f, 255.0f), pc));
@@ -149,26 +153,157 @@ __global__ void raster_resolve_kernel(const float* __restrict__ verts, int nv, i
   }
 }
 
-// one thread per vertex: un-normalised face normals of its incident triangles, added in ascending triangle order
-__global__ void vertex_normal_kernel(const float* __restrict__ v, const int* __restrict__ t, const int* __restrict__ adj_off,
-                                     const int* __restrict__ adj_tri, int nver, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nver) return;
+// the normal of vertex i (_get_normal): un-normalised face normals of its incident triangles, added in ascending triangle
+// order, then divided by their length (1e-6 when it is not positive).  negate_z reads -z (exact: negation commutes with
+// rounding).
+__device__ __forceinline__ void vertex_normal(const float* __restrict__ v, const int* __restrict__ t,
+                                              const int* __restrict__ adj_off, const int* __restrict__ adj_tri, int i,
+                                              bool negate_z, float n[3]) {
   float nx = 0.f, ny = 0.f, nz = 0.f;
   for (int e = adj_off[i]; e < adj_off[i + 1]; ++e) {
     const int tr = adj_tri[e];
     const int a = t[3 * tr], b = t[3 * tr + 1], c = t[3 * tr + 2];
-    const float v1x = rsub(v[3 * b], v[3 * a]), v1y = rsub(v[3 * b + 1], v[3 * a + 1]), v1z = rsub(v[3 * b + 2], v[3 * a + 2]);
-    const float v2x = rsub(v[3 * c], v[3 * a]), v2y = rsub(v[3 * c + 1], v[3 * a + 1]), v2z = rsub(v[3 * c + 2], v[3 * a + 2]);
+    const float za = negate_z ? -v[3 * a + 2] : v[3 * a + 2];
+    const float zb = negate_z ? -v[3 * b + 2] : v[3 * b + 2];
+    const float zc = negate_z ? -v[3 * c + 2] : v[3 * c + 2];
+    const float v1x = rsub(v[3 * b], v[3 * a]), v1y = rsub(v[3 * b + 1], v[3 * a + 1]), v1z = rsub(zb, za);
+    const float v2x = rsub(v[3 * c], v[3 * a]), v2y = rsub(v[3 * c + 1], v[3 * a + 1]), v2z = rsub(zc, za);
     nx = radd(nx, rsub(rmul(v1y, v2z), rmul(v1z, v2y)));
     ny = radd(ny, rsub(rmul(v1z, v2x), rmul(v1x, v2z)));
     nz = radd(nz, rsub(rmul(v1x, v2y), rmul(v1y, v2x)));
   }
   float det = __fsqrt_rn(radd(radd(rmul(nx, nx), rmul(ny, ny)), rmul(nz, nz)));
   if (det <= 0) det = 1e-6f;
-  out[3 * i] = __fdiv_rn(nx, det);
-  out[3 * i + 1] = __fdiv_rn(ny, det);
-  out[3 * i + 2] = __fdiv_rn(nz, det);
+  n[0] = __fdiv_rn(nx, det);
+  n[1] = __fdiv_rn(ny, det);
+  n[2] = __fdiv_rn(nz, det);
+}
+
+// one thread per vertex
+__global__ void vertex_normal_kernel(const float* __restrict__ v, const int* __restrict__ t, const int* __restrict__ adj_off,
+                                     const int* __restrict__ adj_tri, int nver, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nver) return;
+  vertex_normal(v, t, adj_off, adj_tri, i, false, out + 3 * i);
+}
+
+// ---- lighting (Sim3DR/lighting.py:37-63) ----------------------------------------------------------------------------------
+
+// np.clip(x, 0, 1): max(x, 0) then min(., 1), each "a > b ? a : b" with a NaN kept (so clip(-0) = +0 and NaN stays)
+__device__ __forceinline__ float clip01(float x) {
+  if (x != x) return x;
+  const float t = x > 0.f ? x : 0.f;
+  return t < 1.f ? t : 1.f;
+}
+// np.min / np.max reductions propagate NaN
+__device__ __forceinline__ float nan_min(float a, float b) { return (a != a || a < b) ? a : b; }
+__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || a > b) ? a : b; }
+
+// x ** e correctly rounded to float32, e in [0, 16]: the product in double-double (error below 2^-100 relative), then one
+// rounding; a double-double that is exactly a float32 midpoint is resolved by the sign of its low part.
+__device__ __forceinline__ float pow_cr(float x, int e) {
+  if (e == 0) return 1.0f;
+  if (!isfinite(x) || x == 0.f) {                        // zeros, infinities and NaN: the plain product has the exact result
+    float r = x;
+    for (int k = 1; k < e; ++k) r = __fmul_rn(r, x);
+    return r;
+  }
+  const double xd = x;
+  double hi = xd, lo = 0.0;
+  for (int k = 1; k < e; ++k) {                          // (hi, lo) *= x
+    const double p = __dmul_rn(hi, xd);
+    const double err = __fma_rn(lo, xd, __fma_rn(hi, xd, -p));
+    hi = __dadd_rn(p, err);
+    lo = __dsub_rn(err, __dsub_rn(hi, p));
+  }
+  const float f = __double2float_rn(hi);
+  if (!isfinite(hi) || lo == 0.0 || static_cast<double>(f) == hi) return f;
+  // hi lies strictly between f and its neighbour g on hi's side; only an exact midpoint can round the wrong way
+  const float g = nextafterf(f, hi > static_cast<double>(f) ? INFINITY : -INFINITY);
+  const double mid = 0.5 * (static_cast<double>(f) + static_cast<double>(g));
+  if (hi != mid) return f;
+  return ((g > f) == (lo > 0.0)) ? g : f;
+}
+
+__device__ __forceinline__ float block_reduce(float v, bool is_max, float* red) {
+  for (int o = 16; o > 0; o >>= 1) {
+    const float u = __shfl_xor_sync(0xffffffffu, v, o);
+    v = is_max ? nan_max(v, u) : nan_min(v, u);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = red[0];
+  for (int k = 1; k < nw; ++k) v = is_max ? nan_max(v, red[k]) : nan_min(v, red[k]);
+  return v;
+}
+
+// one CTA per head (heads along grid x, strided): the head's per-axis min / max, then every vertex's normal and light.
+// norm_vertices (lighting.py:9-14) needs only those six values: its steps round monotonically, so the global max of
+// v - min is max_a (max_a - min_a), and the per-axis max after "/ M * 2" is that of the per-axis max.
+__global__ void __launch_bounds__(256) light_kernel(const float* __restrict__ verts, int nv, int batch,
+                                                    const int* __restrict__ tris, const int* __restrict__ adj_off,
+                                                    const int* __restrict__ adj_tri, int negate_z, dad3d_lighting L,
+                                                    float* __restrict__ light_out) {
+  __shared__ float red[32];
+  for (int b = blockIdx.x; b < batch; b += gridDim.x) {
+    const float* v = verts + static_cast<long long>(b) * nv * 3;
+    float* out = light_out + static_cast<long long>(b) * nv * 3;
+    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+    for (int i = threadIdx.x; i < nv; i += blockDim.x)
+      for (int a = 0; a < 3; ++a) {
+        const float x = (a == 2 && negate_z) ? -v[3 * i + 2] : v[3 * i + a];
+        lo[a] = nan_min(lo[a], x);
+        hi[a] = nan_max(hi[a], x);
+      }
+    for (int a = 0; a < 3; ++a) {
+      lo[a] = block_reduce(lo[a], false, red);
+      hi[a] = block_reduce(hi[a], true, red);
+    }
+    float span[3], half_top[3];
+    for (int a = 0; a < 3; ++a) span[a] = rsub(hi[a], lo[a]);                       // max(v - min) per axis
+    const float M = nan_max(nan_max(span[0], span[1]), span[2]);                    // vertices.max()
+    for (int a = 0; a < 3; ++a) half_top[a] = __fdiv_rn(rmul(__fdiv_rn(span[a], M), 2.f), 2.f);   // max(0) / 2
+
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+      float n[3];
+      vertex_normal(v, tris, adj_off, adj_tri, i, negate_z != 0, n);
+      float vn[3], light[3] = {0.f, 0.f, 0.f};
+      for (int a = 0; a < 3; ++a) {
+        const float x = (a == 2 && negate_z) ? -v[3 * i + 2] : v[3 * i + a];
+        vn[a] = rsub(rmul(__fdiv_rn(rsub(x, lo[a]), M), 2.f), half_top[a]);
+      }
+      if (L.intensity_ambient > 0)
+        for (int a = 0; a < 3; ++a) light[a] = radd(light[a], rmul(L.intensity_ambient, L.color_ambient[a]));
+      if (L.intensity_directional > 0) {
+        float dir[3];
+        for (int a = 0; a < 3; ++a) dir[a] = rsub(L.light_pos[a], vn[a]);
+        float len = __fsqrt_rn(radd(radd(rmul(dir[0], dir[0]), rmul(dir[1], dir[1])), rmul(dir[2], dir[2])));
+        for (int a = 0; a < 3; ++a) dir[a] = __fdiv_rn(dir[a], len);
+        const float cs = radd(radd(rmul(n[0], dir[0]), rmul(n[1], dir[1])), rmul(n[2], dir[2]));
+        const float cc = clip01(cs);
+        for (int a = 0; a < 3; ++a)
+          light[a] = radd(light[a], rmul(L.intensity_directional, rmul(L.color_directional[a], cc)));
+        if (L.intensity_specular > 0) {
+          float v2v[3];
+          for (int a = 0; a < 3; ++a) v2v[a] = rsub(L.view_pos[a], vn[a]);
+          len = __fsqrt_rn(radd(radd(rmul(v2v[0], v2v[0]), rmul(v2v[1], v2v[1])), rmul(v2v[2], v2v[2])));
+          const float two_cos = rmul(2.f, cs);
+          float spe = 0.f;
+          for (int a = 0; a < 3; ++a) {
+            const float refl = rsub(rmul(two_cos, n[a]), dir[a]);
+            const float p = pow_cr(rmul(__fdiv_rn(v2v[a], len), refl), L.specular_exp);
+            spe = a == 0 ? p : radd(spe, p);
+          }
+          spe = cs != 0.f ? clip01(spe) : 0.f;
+          for (int a = 0; a < 3; ++a)
+            light[a] = radd(light[a], rmul(rmul(L.intensity_specular, L.color_directional[a]), clip01(spe)));
+        }
+      }
+      for (int a = 0; a < 3; ++a) out[3 * i + a] = clip01(light[a]);
+    }
+  }
 }
 
 }  // namespace dad3d
@@ -183,8 +318,8 @@ namespace {
 
 // both entries: `batch` heads drawn into `n_images` images; image_of_head_d NULL is the identity map (n_images = batch)
 int rasterize_mapped(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
-                     const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
-                     const int32_t* image_of_head_d, int32_t n_images, uint8_t* image_d, float* depth_d,
+                     const float* colors_d, long long color_stride, int32_t c, int32_t h, int32_t w, int32_t reverse,
+                     int32_t negate_z, const int32_t* image_of_head_d, int32_t n_images, uint8_t* image_d, float* depth_d,
                      int32_t* tri_index_d, int32_t* head_index_d, unsigned long long* key_ws_d, dad3d_stream stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const size_t hw = static_cast<size_t>(h) * w;
@@ -203,8 +338,20 @@ int rasterize_mapped(const float* vertices_d, int32_t nv, int32_t batch, const i
   DAD3D_CUDA_OK(cudaGetLastError());
   const unsigned int gm = static_cast<unsigned int>(n_images < 65535 ? n_images : 65535);
   raster_resolve_kernel<<<dim3(static_cast<unsigned int>((hw + 255) / 256), gm), 256, 0, stream>>>(
-      vertices_d, nv, n_images, triangles_d, ntri, image_of_head_d ? 1 : 0, colors_d, h, w, c, reverse, negate_z, key_ws_d,
-      image_d, depth_d, tri_index_d, head_index_d);
+      vertices_d, nv, n_images, triangles_d, ntri, image_of_head_d ? 1 : 0, colors_d, color_stride, h, w, c, reverse, negate_z,
+      key_ws_d, image_d, depth_d, tri_index_d, head_index_d);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+int launch_light(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, const int32_t* adj_offsets_d,
+                 const int32_t* adj_triangles_d, int32_t negate_z, const dad3d_lighting& lighting, float* light_d,
+                 cudaStream_t stream) {
+  if (batch == 0) return DAD3D_OK;
+  const unsigned int gx = static_cast<unsigned int>(batch < 65535 ? batch : 65535);
+  light_kernel<<<gx, 256, 0, stream>>>(vertices_d, nv, batch, triangles_d, adj_offsets_d, adj_triangles_d, negate_z, lighting,
+                                       light_d);
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;
@@ -214,6 +361,41 @@ int rasterize_mapped(const float* vertices_d, int32_t nv, int32_t batch, const i
 
 extern "C" {
 
+int dad3d_light_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d,
+                      const int32_t* adj_offsets_d, const int32_t* adj_triangles_d, int32_t negate_z, dad3d_lighting lighting,
+                      float* light_d, dad3d_stream stream) {
+  DAD3D_REQUIRE((vertices_d && triangles_d && adj_offsets_d && adj_triangles_d && light_d) || batch == 0, "null pointer");
+  DAD3D_REQUIRE(batch >= 0 && nv > 0 && static_cast<long long>(nv) * 3 < (1ll << 31), "shape");
+  DAD3D_REQUIRE(lighting.specular_exp >= 0 && lighting.specular_exp <= 16, "specular_exp must be an integer in [0, 16]");
+  return launch_light(vertices_d, nv, batch, triangles_d, adj_offsets_d, adj_triangles_d, negate_z, lighting, light_d,
+                      reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_render_lit(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                     const int32_t* adj_offsets_d, const int32_t* adj_triangles_d, int32_t negate_z, dad3d_lighting lighting,
+                     const int32_t* image_of_head_d, int32_t n_images, int32_t h, int32_t w, float* light_ws_d,
+                     uint8_t* image_d, unsigned long long* key_ws_d, dad3d_stream stream) {
+  DAD3D_REQUIRE(((vertices_d && adj_offsets_d && adj_triangles_d && light_ws_d) || batch == 0) && (triangles_d || ntri == 0) &&
+                    image_d && key_ws_d,
+                "null pointer");
+  DAD3D_REQUIRE(batch >= 0 && nv > 0 && ntri >= 0 && h > 0 && w > 0 && static_cast<long long>(h) * w < (1ll << 31) &&
+                    static_cast<long long>(nv) * 3 < (1ll << 31) && (!image_of_head_d || n_images >= 0),
+                "shape");
+  DAD3D_REQUIRE(lighting.specular_exp >= 0 && lighting.specular_exp <= 16, "specular_exp must be an integer in [0, 16]");
+  DAD3D_REQUIRE(!image_of_head_d || static_cast<unsigned long long>(batch) * static_cast<unsigned long long>(ntri) <=
+                                        0xFFFFFFFEull,
+                "batch * ntri exceeds 2^32 - 2");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (ntri > 0) {                                       // without triangles nothing is drawn and the light is not needed
+    const int rc = launch_light(vertices_d, nv, batch, triangles_d, adj_offsets_d, adj_triangles_d, negate_z, lighting,
+                                light_ws_d, st);
+    if (rc != DAD3D_OK) return rc;
+  }
+  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, light_ws_d, static_cast<long long>(nv) * 3, 3, h, w, 0,
+                          negate_z, image_of_head_d, image_of_head_d ? n_images : batch, image_d, nullptr, nullptr, nullptr,
+                          key_ws_d, stream);
+}
+
 int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
                           const float* colors_d, int32_t c, int32_t h, int32_t w, int32_t reverse, int32_t negate_z,
                           uint8_t* image_d, float* depth_d, int32_t* tri_index_d, unsigned long long* key_ws_d,
@@ -222,7 +404,7 @@ int dad3d_rasterize_batch(const float* vertices_d, int32_t nv, int32_t batch, co
   DAD3D_REQUIRE(!image_d || colors_d, "image_d needs colors_d");
   DAD3D_REQUIRE(batch >= 0 && nv > 0 && ntri >= 0 && h > 0 && w > 0 && c > 0 && static_cast<long long>(h) * w < (1ll << 31),
                 "shape");
-  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, c, h, w, reverse, negate_z, nullptr, batch,
+  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, 0, c, h, w, reverse, negate_z, nullptr, batch,
                           image_d, depth_d, tri_index_d, nullptr, key_ws_d, stream);
 }
 
@@ -238,7 +420,7 @@ int dad3d_rasterize_frames(const float* vertices_d, int32_t nv, int32_t batch, c
   // the key's low word holds ~(head * ntri + triangle): every pair must stay below 2^32 - 1
   DAD3D_REQUIRE(static_cast<unsigned long long>(batch) * static_cast<unsigned long long>(ntri) <= 0xFFFFFFFEull,
                 "batch * ntri exceeds 2^32 - 2");
-  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, c, h, w, 0, negate_z, image_of_head_d, n_images,
+  return rasterize_mapped(vertices_d, nv, batch, triangles_d, ntri, colors_d, 0, c, h, w, 0, negate_z, image_of_head_d, n_images,
                           image_d, depth_d, tri_index_d, head_index_d, key_ws_d, stream);
 }
 

@@ -6,8 +6,9 @@ stages and their helper names, so ``demo.py`` / ``demo_utils.py`` code written a
 What changes is where the arithmetic runs: ``self.model`` is the CUDA encoder (csrc/encoder.cu) instead of a TorchScript
 module, and ``self.head_mesh`` decodes on the GPU (csrc/flame.cu), once instead of twice per image.
 ``predict_batch`` is the batched, device-resident entry point the reference does not have (SURVEY §8b); with ``render`` it
-also draws the PNCC, depth and triangle-index maps of every head (rasterizer.PnccRenderer) inside the same step, and with
-``boxes`` plus ``frame_render`` the same maps of every whole frame, all its heads in one z-buffer.
+also draws the PNCC, depth and triangle-index maps of every head (rasterizer.PnccRenderer) and its lit render
+(rasterizer.LitRenderer, the reference's Sim3DR RenderPipeline) inside the same step, and with ``boxes`` plus
+``frame_render`` the same maps of every whole frame, all its heads in one z-buffer.
 """
 from __future__ import annotations
 
@@ -24,7 +25,7 @@ from . import _lib
 from .encoder import OUTPUT_2D_LANDMARKS, OUTPUT_3DMM_PARAMS, OUTPUT_LANDMARKS_HEATMAP, Dad3dEncoder
 from .flame import load_flame_static
 from .head_mesh import HeadMesh
-from .rasterizer import PnccRenderer
+from .rasterizer import LitRenderer, PnccRenderer
 
 logger = logging.getLogger(__name__)
 ROI_RECORD_BYTES = 72                                # sizeof(dad3d_roi), include/dad3d.h
@@ -32,8 +33,8 @@ MAX_ROIS = 65535                                     # ROIs per call: dad3d_prep
 _FILENAME = "dad_3dheads.trcd"
 _MEAN = (0.485, 0.456, 0.406)
 _STD = (0.229, 0.224, 0.225)
-RENDER_KEYS = ("pncc", "depth", "tri_index")
-FRAME_RENDER_KEYS = ("pncc", "depth", "tri_index", "head_index")    # predict_batch(boxes=, frame_render=) -> "frame_<key>"
+RENDER_KEYS = ("pncc", "depth", "tri_index", "lit")
+FRAME_RENDER_KEYS = ("pncc", "depth", "tri_index", "head_index", "lit")    # predict_batch(boxes=, frame_render=) -> "frame_<key>"
 
 DEFAULT_CONFIG = {                                   # == the reference's dad_3dnet.yaml
     "model_path": ".dad_checkpoints/dad_3dheads.trcd",
@@ -125,6 +126,7 @@ class FaceMeshPredictor:
         self._lm_index: Dict[str, Tensor] = {}
         self._graphs: Dict[Any, Any] = {}
         self._renderer: Optional[PnccRenderer] = None
+        self._lit_renderer: Optional[LitRenderer] = None
 
     # ------------------------------------------------------------------ reference single-image API
     def __call__(self, x: Any) -> Any:
@@ -307,6 +309,11 @@ class FaceMeshPredictor:
             self._renderer = PnccRenderer(self.device)
         return self._renderer
 
+    def _lit(self) -> LitRenderer:
+        if self._lit_renderer is None:                       # the reference's default lighting; tables uploaded once
+            self._lit_renderer = LitRenderer(self.device)
+        return self._lit_renderer
+
     def _check_rois(self, frames, boxes, frame_index) -> Tuple[Tensor, Optional[Tensor]]:
         """Validates the frames + boxes arguments before anything is launched -> (boxes, frame_index) as tensors."""
         if not (isinstance(frames, Tensor) and frames.dtype == torch.uint8 and frames.ndim == 4 and frames.shape[3] == 3):
@@ -372,11 +379,14 @@ class FaceMeshPredictor:
             out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
         if frame_render:
             frame_of_head = torch.where(out["valid"], fields[:, 4], -1)            # invalid boxes draw nothing
-            maps = self._pncc_renderer().render_frames(proj, frame_of_head, F, (H, W), pncc="pncc" in frame_render,
-                                                       depth="depth" in frame_render,
-                                                       tri_index="tri_index" in frame_render,
-                                                       head_index="head_index" in frame_render)
-            out.update({f"frame_{k}": t for k, t in maps.items()})
+            if set(frame_render) - {"lit"}:
+                maps = self._pncc_renderer().render_frames(proj, frame_of_head, F, (H, W), pncc="pncc" in frame_render,
+                                                           depth="depth" in frame_render,
+                                                           tri_index="tri_index" in frame_render,
+                                                           head_index="head_index" in frame_render)
+                out.update({f"frame_{k}": t for k, t in maps.items()})
+            if "lit" in frame_render:
+                out["frame_lit"] = self._lit().render_frames(proj, frame_of_head, F, (H, W), frames=frames)["lit"]
         return out
 
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
@@ -388,9 +398,11 @@ class FaceMeshPredictor:
         "3dmm_params" [B,413], "points" [B,68,2] (pixels of the 256x256 network input), "3d_vertices" [B,5023,3],
         "projected_vertices" [B,5023,2|3], "landmarks_<subset>" [B,L,2|3].
 
-        ``render``: a subset of ("pncc", "depth", "tri_index") (needs ``to_2d=False``) adds those maps of every head, drawn
-        by :class:`~dad_3dheads_b200.rasterizer.PnccRenderer` from "projected_vertices" at the network input size, in the
-        frame of "points": "pncc" [B,S,S,3] uint8, "depth" [B,S,S] fp32, "tri_index" [B,S,S] int32.
+        ``render``: a subset of ("pncc", "depth", "tri_index", "lit") (needs ``to_2d=False``) adds those maps of every
+        head, drawn by :class:`~dad_3dheads_b200.rasterizer.PnccRenderer` from "projected_vertices" at the network input
+        size, in the frame of "points": "pncc" [B,S,S,3] uint8, "depth" [B,S,S] fp32, "tri_index" [B,S,S] int32; "lit"
+        [B,S,S,3] uint8 is the reference's ``RenderPipeline()`` shaded head on black, with its default lighting
+        (:class:`~dad_3dheads_b200.rasterizer.LitRenderer`; other lights: a LitRenderer on "projected_vertices").
 
         ``boxes``: heads in whole frames.  ``images`` is then one [F,H,W,3] uint8 tensor of frames and ``boxes`` an [R,4]
         integer tensor of head boxes [x, y, w, h] in frame pixels (host or device), on frame ``frame_index[r]`` ([R]
@@ -407,7 +419,11 @@ class FaceMeshPredictor:
         those maps of every whole frame, all its valid boxes' heads drawn from "projected_vertices" into one image and one
         z-buffer (:meth:`~dad_3dheads_b200.rasterizer.PnccRenderer.render_frames`): "frame_pncc" [F,H,W,3] uint8,
         "frame_depth" [F,H,W] fp32 (-z; -1e8 for background), "frame_tri_index" [F,H,W] int32 (the triangle within its
-        head) and "frame_head_index" [F,H,W] int32 (the box), -1 for background.  A frame equals the reference's
+        head) and "frame_head_index" [F,H,W] int32 (the box), -1 for background; "frame_lit" [F,H,W,3] uint8, the heads
+        shaded by the reference's default ``RenderPipeline()`` drawn over the frames (it takes ``bg``): each head lit on
+        its own, then composited with one z-buffer per frame by the same rule (:meth:`LitRenderer.render_frames
+        <dad_3dheads_b200.rasterizer.LitRenderer.render_frames>`; not a loop of RenderPipeline calls, whose fresh depth
+        buffers would let a later box paint over a nearer earlier one).  A frame's PNCC maps equal the reference's
         ``PNCCEstimator()(frame, {"3dmm_params": p})`` run for its boxes' frame-space parameters one after the other in box
         order on the same buffers: the nearest head wins, an exact depth tie goes to the earlier box, invalid boxes draw
         nothing.  The reference's ``with_background=True`` overlay is, exactly,
@@ -430,9 +446,11 @@ class FaceMeshPredictor:
         if landmark_subset is not None:
             dec = self.head_mesh.flame.decoder(self.device)
             out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
-        if render:
+        if set(render) - {"lit"}:
             out.update(self._pncc_renderer()(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
                                       tri_index="tri_index" in render))
+        if "lit" in render:
+            out.update(self._lit()(proj, self._img_size))
         return out
 
     def _ws_generation(self):

@@ -6,7 +6,11 @@ the reference's ``inference/pncc_estimator.py`` through ``compat/Sim3DR``.  No C
 tensors in and out, no host synchronisation (so they run inside a captured CUDA graph); every head equals, bit for bit, what
 ``rasterize`` gives for that head alone.  With a head -> image map (``rasterize_batch(image_of_head=, num_images=)``,
 ``PnccRenderer.render_frames``) several heads share one image and one z-buffer, as when a caller of the reference draws the
-heads of a whole frame one after the other into the same buffers."""
+heads of a whole frame one after the other into the same buffers.
+
+``light_batch`` and ``LitRenderer`` are the reference's ``Sim3DR.RenderPipeline`` (Sim3DR/lighting.py:23-71) in the same
+batched form: per-vertex ambient, diffuse and specular light of every head, then the rasteriser with each head's light as
+its colours."""
 from __future__ import annotations
 
 import os
@@ -251,3 +255,189 @@ class PnccRenderer:
         if pncc:
             out["pncc"] = out.pop("image")
         return out
+
+
+# RenderPipeline's keyword arguments and defaults (Sim3DR/lighting.py:24-32)
+LIGHTING_DEFAULTS = {"intensity_ambient": 0.3, "intensity_directional": 0.6, "intensity_specular": 0.1, "specular_exp": 5,
+                     "color_ambient": (1, 1, 1), "color_directional": (1, 1, 1), "light_pos": (0, 0, 5),
+                     "view_pos": (0, 0, 5)}
+MAX_SPECULAR_EXP = 16
+
+
+def lighting_struct(lighting: Optional[dict] = None) -> _lib.Lighting:
+    """RenderPipeline keyword arguments (None or missing keys: the reference's defaults) -> the ``dad3d_lighting`` the
+    kernel takes.  Intensities are scalars, colours and positions 3-sequences, all used as float32 as the reference's
+    float32 arithmetic does; ``specular_exp`` must be an integer in [0, 16] (the device computes the correctly rounded power
+    only for those).  Raises ValueError otherwise."""
+    kw = dict(LIGHTING_DEFAULTS)
+    unknown = set(lighting or {}) - set(kw)
+    if unknown:
+        raise ValueError(f"unknown lighting arguments {sorted(unknown)}; choose from {sorted(kw)}")
+    kw.update(lighting or {})
+    e = kw["specular_exp"]
+    if isinstance(e, (bool, np.bool_)) or not isinstance(e, (int, np.integer)) or not 0 <= int(e) <= MAX_SPECULAR_EXP:
+        raise ValueError(f"specular_exp must be an integer in [0, {MAX_SPECULAR_EXP}], got {e!r}")
+    L = _lib.Lighting()
+    for k in ("intensity_ambient", "intensity_directional", "intensity_specular"):
+        x = float(kw[k])
+        if x > 0 and np.float32(x) <= 0:       # the reference tests "> 0" before rounding to float32
+            raise ValueError(f"{k}={x!r} is positive but rounds to 0 in float32")
+        setattr(L, k, float(np.float32(x)))
+    L.specular_exp = int(e)
+    for k in ("color_ambient", "color_directional", "light_pos", "view_pos"):
+        a = np.asarray(kw[k], dtype=np.float32).reshape(-1)
+        if a.shape != (3,):
+            raise ValueError(f"{k} must have 3 components, got {kw[k]!r}")
+        getattr(L, k)[:] = [float(x) for x in a]
+    return L
+
+
+def _adjacency(triangles: torch.Tensor, nv: int):
+    """The CSR vertex -> triangle lists of ``triangles`` on its device, built on the host once per tensor and content
+    version (the first call synchronises; later calls, e.g. inside a capture after the warm-up, do not)."""
+    tag = (nv, triangles._version)
+    cached = getattr(triangles, "_dad3d_adj", None)
+    if cached is not None and cached[0] == tag:
+        return cached[1]
+    off, adj = vertex_adjacency(triangles.cpu().numpy(), nv)
+    pair = (torch.from_numpy(off).to(triangles.device), torch.from_numpy(adj).to(triangles.device))
+    triangles._dad3d_adj = (tag, pair)
+    return pair
+
+
+def _check_mesh(vertices: torch.Tensor, triangles: torch.Tensor):
+    if vertices.ndim != 3 or vertices.shape[2] != 3 or vertices.dtype != torch.float32 or not vertices.is_cuda:
+        raise ValueError("vertices must be a [B,nv,3] float32 CUDA tensor")
+    if triangles.ndim != 2 or triangles.shape[1] != 3 or triangles.dtype != torch.int32 or triangles.device != vertices.device:
+        raise ValueError("triangles must be an [ntri,3] int32 tensor on the vertices' device")
+    nv = int(vertices.shape[1])
+    if nv == 0 or 3 * nv >= 1 << 31:
+        raise ValueError(f"bad vertex count {nv}")
+    triangles = triangles.contiguous()
+    _check_triangles(triangles, nv)
+    return vertices.contiguous(), triangles
+
+
+def light_batch(vertices: torch.Tensor, triangles: torch.Tensor, *, lighting: Optional[dict] = None,
+                negate_z: bool = False) -> torch.Tensor:
+    """RenderPipeline's per-vertex ``light`` (Sim3DR/lighting.py:38-63) of B heads on the GPU (``dad3d_light_batch``).
+
+    vertices [B,nv,3] float32 (with ``negate_z``, -z is used, as the predictor's renders do), triangles [ntri,3] int32 on
+    the same device, ``lighting`` RenderPipeline's keyword arguments (:func:`lighting_struct`).  Returns [B,nv,3] float32 in
+    [0,1] (NaN where the reference's arithmetic gives NaN).  Every head is lit on its own: norm_vertices uses that head's
+    extent.  Every float32 operation is the reference's, in its order; (v2v * reflection) ** specular_exp is the correctly
+    rounded power, which the reference's ``np.power`` misses by one ulp for some inputs.  No host synchronisation except
+    the first use of a ``triangles`` tensor (bounds check and adjacency)."""
+    L = lighting_struct(lighting)
+    vertices, triangles = _check_mesh(vertices, triangles)
+    B, nv = int(vertices.shape[0]), int(vertices.shape[1])
+    off, adj = _adjacency(triangles, nv)
+    out = torch.empty(B, nv, 3, dtype=torch.float32, device=vertices.device)
+    lib = _lib.load()
+    with torch.cuda.device(vertices.device):
+        _lib.check(lib.dad3d_light_batch(vertices.data_ptr(), nv, B, triangles.data_ptr(), off.data_ptr(), adj.data_ptr(),
+                                         1 if negate_z else 0, L, out.data_ptr(),
+                                         torch.cuda.current_stream(vertices.device).cuda_stream), "dad3d_light_batch")
+    return out
+
+
+def render_lit(vertices: torch.Tensor, triangles: torch.Tensor, *, height: int, width: int, lighting: Optional[dict] = None,
+               negate_z: bool = False, image: Optional[torch.Tensor] = None, image_of_head: Optional[torch.Tensor] = None,
+               num_images: Optional[int] = None) -> torch.Tensor:
+    """Lit render of B heads (``dad3d_render_lit``): :func:`light_batch`, then the z-buffer rasteriser with each head's light
+    as its colours, alpha = 1.  Returns [N,height,width,3] uint8: zeros, or a copy of ``image`` ([N,height,width,3] uint8),
+    with the heads drawn over it.  Without ``image_of_head`` N = B and image b is RenderPipeline()(head b, triangles, bg)
+    exactly.  With ``image_of_head`` ([B] int32 on the device) and ``num_images`` = N, as :func:`rasterize_batch`: each head
+    is lit on its own, then all heads of an image share one z-buffer, the nearest surface wins and an exact tie goes to the
+    lower head; heads mapped outside [0, N) draw nothing.  That is the reference's ``_rasterize`` run once on the union mesh
+    with the heads' lights as colours, NOT a loop of RenderPipeline calls (each call starts a fresh depth buffer, so a later
+    head would paint over a nearer earlier one)."""
+    L = lighting_struct(lighting)
+    vertices, triangles = _check_mesh(vertices, triangles)
+    dev = vertices.device
+    B, nv, ntri = int(vertices.shape[0]), int(vertices.shape[1]), int(triangles.shape[0])
+    height, width = int(height), int(width)
+    if height <= 0 or width <= 0 or height * width >= 1 << 31:
+        raise ValueError(f"bad image size {height} x {width}")
+    mapped = image_of_head is not None
+    if mapped != (num_images is not None):
+        raise ValueError("image_of_head and num_images go together")
+    n_out = B
+    if mapped:
+        if image_of_head.shape != (B,) or image_of_head.dtype != torch.int32 or image_of_head.device != dev:
+            raise ValueError(f"image_of_head must be a [{B}] int32 tensor on the vertices' device")
+        n_out = int(num_images)
+        if n_out < 0:
+            raise ValueError(f"num_images must be >= 0, got {n_out}")
+        if B * ntri > 2 ** 32 - 2:
+            raise ValueError(f"{B} heads x {ntri} triangles exceed 2^32 - 2 (head, triangle) pairs")
+        image_of_head = image_of_head.contiguous()
+    if image is None:
+        out = torch.zeros(n_out, height, width, 3, dtype=torch.uint8, device=dev)
+    else:
+        if tuple(image.shape) != (n_out, height, width, 3) or image.dtype != torch.uint8:
+            raise ValueError(f"image must be [{n_out},{height},{width},3] uint8")
+        out = image.to(dev, copy=True).contiguous()
+    if B == 0 or n_out == 0:
+        return out
+    off, adj = _adjacency(triangles, nv)
+    light = torch.empty(B * nv * 3, dtype=torch.float32, device=dev)            # caching allocator: capture-safe
+    key = torch.empty(max(n_out, 1) * height * width, dtype=torch.int64, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        _lib.check(lib.dad3d_render_lit(vertices.data_ptr(), nv, B, triangles.data_ptr(), ntri, off.data_ptr(),
+                                        adj.data_ptr(), 1 if negate_z else 0, L,
+                                        image_of_head.data_ptr() if mapped else None, n_out, height, width,
+                                        light.data_ptr(), out.data_ptr(), key.data_ptr(),
+                                        torch.cuda.current_stream(dev).cuda_stream), "dad3d_render_lit")
+    return out
+
+
+class LitRenderer:
+    """The reference's ``RenderPipeline(**lighting)`` (Sim3DR/lighting.py:23-71) for a batch of decoded heads, drawn as
+    the predictor's PNCC render draws them: z negated (a larger -z is nearer), on a black background.
+
+    ``triangles`` None means the PNCC faces without ears with the winding reversed (``faces_wo_ears[:, [0, 2, 1]]``):
+    negating z reflects the mesh, which reverses the orientation of FLAME's counter-clockwise faces, so their normals would
+    face away from the light at +z (DESIGN §4.6).  Lighting keyword arguments as RenderPipeline's (:func:`lighting_struct`).
+    Adjacency and tables are uploaded once, so both methods are safe inside a CUDA graph capture after one warm-up call;
+    neither synchronises the host."""
+
+    def __init__(self, device=None, triangles=None, **lighting):
+        if not torch.cuda.is_available():
+            raise _lib.Dad3dError("LitRenderer needs a CUDA (sm_90a) device: there is no CPU path")
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.lighting = dict(lighting)
+        lighting_struct(self.lighting)                          # validate now, before any launch
+        st = load_render_static()
+        self.nv = int(st["ncc_colors"].shape[0])
+        if triangles is None:
+            triangles = st["faces_wo_ears"][:, [0, 2, 1]]
+        self.faces = torch.as_tensor(np.ascontiguousarray(np.asarray(triangles), dtype=np.int32)).to(self.device)
+        _check_triangles(self.faces, self.nv)
+        _adjacency(self.faces, self.nv)
+
+    def _check(self, v: torch.Tensor) -> None:
+        if v.ndim != 3 or v.shape[1:] != (self.nv, 3):
+            raise ValueError(f"expected [B,{self.nv},3] vertices, got {tuple(v.shape)}")
+
+    def __call__(self, projected_vertices_3d: torch.Tensor, size: int) -> Dict[str, torch.Tensor]:
+        """[B,5023,3] float32 on the device (``HeadMesh.decode(..., to_2d=False)``) -> {"lit": [B,S,S,3] uint8}, each head
+        equal to ``RenderPipeline(**lighting)(v, triangles, zeros)`` with z negated."""
+        self._check(projected_vertices_3d)
+        return {"lit": render_lit(projected_vertices_3d, self.faces, height=size, width=size, lighting=self.lighting,
+                                  negate_z=True)}
+
+    def render_frames(self, projected_vertices_3d: torch.Tensor, frame_of_head: torch.Tensor, num_frames: int, size,
+                      frames: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        """B heads in frame pixels into ``num_frames`` frames of ``size`` = (H, W): {"lit": [F,H,W,3] uint8}, drawn over a
+        copy of ``frames`` ([F,H,W,3] uint8) or over black.  ``frame_of_head`` [B] int32 on the device names each head's
+        frame; entries outside [0, F) draw nothing.  Each head is lit by its own RenderPipeline, which normalises that
+        head's vertices; then the heads of a frame share one z-buffer: the nearest surface wins and an exact depth tie goes
+        to the earlier head, the rule of ``PnccRenderer.render_frames``.  This is the reference's ``_rasterize`` run once
+        on the union mesh with the heads' lights as colours.  It is not a loop of RenderPipeline calls, where each call
+        starts a fresh depth buffer and a later head paints over a nearer earlier one."""
+        self._check(projected_vertices_3d)
+        height, width = (int(v) for v in size)
+        return {"lit": render_lit(projected_vertices_3d, self.faces, height=height, width=width, lighting=self.lighting,
+                                  negate_z=True, image=frames, image_of_head=frame_of_head, num_images=num_frames)}

@@ -328,7 +328,25 @@ DAD3D_API int dad3d_allgather_outputs(dad3d_comm* c, const void* send_d, void* r
  *     pair in 32 bits).  batch = 0 or ntri = 0 launches nothing and sets the index maps to -1 (with batch = 0, vertices_d
  *     and image_of_head_d may be NULL).
  *   dad3d_vertex_normals: normalised sum of the incident (un-normalised) face normals per vertex; adj_offsets_d [nv+1] /
- *     adj_triangles_d = CSR list of each vertex's triangles in ascending order (fixed per topology). */
+ *     adj_triangles_d = CSR list of each vertex's triangles in ascending order (fixed per topology).
+ *
+ * Lit meshes: the reference's Sim3DR RenderPipeline (Sim3DR/lighting.py:23-71), per-vertex ambient + diffuse + specular
+ * light of each head, then the rasteriser above with each head's light as its colours.
+ *   dad3d_light_batch: light_d [batch,nv,3] fp32 = RenderPipeline's `light` of every head (vertices_d [batch,nv,3], -z when
+ *     negate_z != 0), every float32 operation in the reference's order, round-to-nearest, no contraction: the normal of
+ *     dad3d_vertex_normals, norm_vertices from the head's per-axis min / max, the diffuse and specular terms, the final clip
+ *     (NaN propagates as np.clip does).  One exception: (v2v * reflection) ** specular_exp is the correctly rounded float32
+ *     power, and specular_exp must be an integer in [0, 16] (else DAD3D_ERR_INVALID).  One CTA per head.
+ *   dad3d_render_lit: dad3d_light_batch into light_ws_d [batch*nv*3] fp32, then the two raster passes with each head's light
+ *     as colours, alpha = 1, into image_d (uint8, c = 3, read-modify-write: zeros or a background).  image_of_head_d NULL:
+ *     image_d is [batch,h,w,3], one image per head (n_images ignored); else as dad3d_rasterize_frames, [n_images,h,w,3] with
+ *     one z-buffer per image, and batch * ntri must stay <= 2^32 - 2.  key_ws_d = (mapped ? n_images : batch)*h*w 64-bit
+ *     words.  Every argument is checked before the first launch. */
+typedef struct dad3d_lighting {
+  float intensity_ambient, intensity_directional, intensity_specular; /* a term is skipped unless its intensity is > 0 */
+  int32_t specular_exp;                                              /* 0..16 */
+  float color_ambient[3], color_directional[3], light_pos[3], view_pos[3];
+} dad3d_lighting;
 DAD3D_API int dad3d_rasterize(const float* vertices_d, const int32_t* triangles_d, const float* colors_d, int32_t ntri,
                               uint8_t* image_d, float* depth_d, unsigned long long* key_ws_d, int32_t h, int32_t w, int32_t c,
                               int32_t reverse, dad3d_stream stream);
@@ -343,6 +361,13 @@ DAD3D_API int dad3d_rasterize_frames(const float* vertices_d, int32_t nv, int32_
                                      dad3d_stream stream);
 DAD3D_API int dad3d_vertex_normals(const float* vertices_d, const int32_t* triangles_d, const int32_t* adj_offsets_d,
                                    const int32_t* adj_triangles_d, int32_t nver, float* normals_d, dad3d_stream stream);
+DAD3D_API int dad3d_light_batch(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d,
+                                const int32_t* adj_offsets_d, const int32_t* adj_triangles_d, int32_t negate_z,
+                                dad3d_lighting lighting, float* light_d, dad3d_stream stream);
+DAD3D_API int dad3d_render_lit(const float* vertices_d, int32_t nv, int32_t batch, const int32_t* triangles_d, int32_t ntri,
+                               const int32_t* adj_offsets_d, const int32_t* adj_triangles_d, int32_t negate_z,
+                               dad3d_lighting lighting, const int32_t* image_of_head_d, int32_t n_images, int32_t h, int32_t w,
+                               float* light_ws_d, uint8_t* image_d, unsigned long long* key_ws_d, dad3d_stream stream);
 
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
