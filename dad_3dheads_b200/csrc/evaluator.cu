@@ -120,6 +120,9 @@ __global__ void align_kernel(const float* __restrict__ v, int nv, int B, const f
   for (int c = 0; c < 3; ++c) out[3 * i + c] = fmaf(s, fmaf(x, R[c], fmaf(y, R[3 + c], z * R[6 + c])), trans[3 * h + c]);
 }
 
+// both batched kernels put the head on grid.y, which holds at most 65535 blocks: larger batches run in slices of heads
+constexpr int32_t kMaxGridY = 65535;
+
 }  // namespace dad3d
 
 using namespace dad3d;
@@ -132,10 +135,13 @@ int dad3d_eval_chamfer(const float* a_d, int32_t na, const float* b_d, int32_t n
   if (B == 0) return DAD3D_OK;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DAD3D_CUDA_OK(cudaMemsetAsync(out_d, 0, sizeof(float) * B, stream));
-  dim3 grid((na + 255) / 256, B);
-  chamfer_kernel<<<grid, 256, 0, stream>>>(a_d, na, b_d, nb, out_d);
-  count_launch();
-  DAD3D_CUDA_OK(cudaGetLastError());
+  for (int32_t h0 = 0; h0 < B; h0 += kMaxGridY) {
+    const int32_t n = B - h0 < kMaxGridY ? B - h0 : kMaxGridY;
+    chamfer_kernel<<<dim3((na + 255) / 256, n), 256, 0, stream>>>(a_d + static_cast<size_t>(h0) * na * 3, na,
+                                                                  b_d + static_cast<size_t>(h0) * nb * 3, nb, out_d + h0);
+    count_launch();
+    DAD3D_CUDA_OK(cudaGetLastError());
+  }
   return DAD3D_OK;
 }
 
@@ -145,10 +151,13 @@ int dad3d_eval_zn(const float* pred_d, const float* gt_d, int32_t K, int32_t B, 
   if (B == 0) return DAD3D_OK;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DAD3D_CUDA_OK(cudaMemsetAsync(out_d, 0, sizeof(float) * B, stream));
-  dim3 grid(top_k, B);
-  zn_kernel<<<grid, 1024, 0, stream>>>(pred_d, gt_d, K, top_k, out_d);
-  count_launch();
-  DAD3D_CUDA_OK(cudaGetLastError());
+  for (int32_t h0 = 0; h0 < B; h0 += kMaxGridY) {
+    const int32_t n = B - h0 < kMaxGridY ? B - h0 : kMaxGridY;
+    const size_t off = static_cast<size_t>(h0) * K * 3;
+    zn_kernel<<<dim3(top_k, n), 1024, 0, stream>>>(pred_d + off, gt_d + off, K, top_k, out_d + h0);
+    count_launch();
+    DAD3D_CUDA_OK(cudaGetLastError());
+  }
   return DAD3D_OK;
 }
 

@@ -47,26 +47,33 @@ def test_gpu_evaluator_matches_oracle_and_reference(cuda_device, tmp_path):
                 assert abs(got - v) <= 1e-4 * abs(v) + 1e-6
 
 
+
 def test_zn_kernel_exact_on_well_separated_points(cuda_device):
-    """calc_zn bit-for-bit on inputs without near-ties (random points: distinct distances)."""
+    """calc_zn exactly, on points whose squared distances to every centre differ pairwise by more than 3e-5 (so that
+    torch.cdist's rounding cannot reorder them): the count recovered from the output is the reference's, and the output
+    is within top_k ulps of its value (the kernel adds one term per column with atomics, in any order)."""
     from dad_3dheads_b200.evaluator import DADEvaluatorGPU
     from oracle.evaluator_oracle import calc_zn
+    from tests import eval_model as em
     ev = DADEvaluatorGPU()
     g = torch.Generator().manual_seed(0)
     for K in (64, 1000, 3669):
-        gt = torch.randn(3, K, 3, generator=g)
-        pred = gt + 0.3 * torch.randn(3, K, 3, generator=g)
-        got = ev.calc_zn(pred.to(cuda_device), gt.to(cuda_device), 5).cpu()
-        want = torch.tensor([calc_zn(pred[b], gt[b], 5) for b in range(3)])
-        assert (got - want).abs().max() < 5e-4, (K, got, want)
+        for top_k in (1, 5, 16):
+            gt = torch.stack([em.separated_points(K, top_k, seed=K + top_k + 100 * b) for b in range(3)])
+            pred = gt + 0.3 * torch.randn(3, K, 3, generator=g)
+            got = ev.calc_zn(pred.to(cuda_device), gt.to(cuda_device), top_k).cpu()
+            want = torch.tensor([calc_zn(pred[b], gt[b], top_k) for b in range(3)])
+            n = K * top_k
+            assert torch.equal(torch.round(got.double() * n), torch.round(want.double() * n)), (K, top_k, got, want)
+            assert ((got.double() - want.double()).abs() <= top_k * em.ulp(want)).all(), (K, top_k, got, want)
 
 
 def test_chamfer_kernel(cuda_device):
+    """Against the float64 definition (the exact tests compare with the fp32 model): every 7th point of a lies on b."""
     from dad_3dheads_b200.evaluator import DADEvaluatorGPU
+    from tests import eval_model as em
     ev = DADEvaluatorGPU()
-    g = torch.Generator().manual_seed(1)
-    a = torch.randn(4, 2094, 3, generator=g)
-    b = torch.randn(4, 5023, 3, generator=g)
+    a, b = em.chamfer_inputs(2094, 5023, 4, seed=1)
     got = ev.chamfer_one_sided(a.to(cuda_device), b.to(cuda_device)).cpu()
     want = (torch.cdist(a.double(), b.double()) ** 2).min(dim=2).values.mean(dim=1)
     assert ((got.double() - want).abs() / want).max() < 1e-5

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from oracle.flame_oracle import FLAME_CONSTS, FlameOracle, sample_params, synthetic_static
+from tests import eval_model
 
 pytestmark = pytest.mark.gpu
 
@@ -240,8 +241,8 @@ def test_landmark_gathers(head_mesh, flame_static, cuda_device):
     tri = faces[fi]
     bary = torch.from_numpy(flame_static["static_lmk_b_coords"])
     got = dec.gather_bary(pj, tri, bary)
-    want = (pj.cpu()[:, tri] * bary[None, :, :, None]).sum(2)
-    assert torch.allclose(got.cpu(), want, atol=1e-4, rtol=1e-6)
+    want = eval_model.gather_bary(pj.cpu(), tri, bary.float())
+    assert torch.equal(got.cpu().view(torch.int32), want.view(torch.int32))
     assert dec.gather(pj, torch.zeros(0, dtype=torch.int64)).shape == (6, 0, 2)
 
 
