@@ -57,6 +57,12 @@ SIGNATURES = {
     "dad3d_flame_backward_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
     "dad3d_flame_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_float,
                                         C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_flame_backward_blend": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "dad3d_flame_backward_vertex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_float,
+                                               C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_flame_backward_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "dad3d_flame_backward_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_gather_landmarks": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                           C.c_void_p, C.c_void_p]),
     "dad3d_gather_landmarks_bary": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,

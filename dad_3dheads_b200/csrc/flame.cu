@@ -610,10 +610,14 @@ __device__ void head_transforms_dual(const Dual* jaw, const Dual* rot6, const Du
   for (int r = 0; r < 3; ++r) out[24 + r] = kMeshOffsetZ * R6[3 * r + 2];
 }
 
-// per head: max |g_v| over the mesh (g = gV + (image/2) sc gP) -> the power-of-two factor that lifts dp into the fp16 range
+// per head: max |g_v| over the mesh (g = gV + (image/2) sc gP) -> the power-of-two factor that lifts dp into the fp16 range.
+// The exponent is capped at sigma_emax = min(127, 127 - log2(basis_scale)), so that sigma and lift = sigma * basis_scale stay
+// finite and unlift = 1 / lift is its exact reciprocal: a head whose gradient is below ~2^(log2(basis_scale) - 118) is lifted
+// less than to [512, 1024) (its dp may land among the fp16 subnormals) instead of by an infinite factor (0 * inf = NaN).
+// NaN gradient entries do not raise the maximum (fmaxf); an infinite maximum gives sigma = 1.
 __global__ void __launch_bounds__(256)
 flame_bwd_gmax_kernel(const float* __restrict__ gv, const float* __restrict__ gp, int pc, int nv, const float* __restrict__ xf,
-                      float half_img, float* __restrict__ sigma) {
+                      float half_img, int sigma_emax, float* __restrict__ sigma) {
   const int h = blockIdx.x;
   const float sc = xf[static_cast<size_t>(h) * kXfFloats + 63] * half_img;
   float m = 0.f;
@@ -634,7 +638,7 @@ flame_bwd_gmax_kernel(const float* __restrict__ gv, const float* __restrict__ gp
     float s = 1.f;
     if (m > 0.f && isfinite(m)) {
       frexpf(m, &e);                                   // m = f * 2^e, f in [0.5, 1)
-      s = ldexpf(1.f, 10 - e);                         // sigma * m in [512, 1024)
+      s = ldexpf(1.f, min(10 - e, sigma_emax));        // sigma * m in [512, 1024) unless capped
     }
     sigma[h] = s;
   }
@@ -1354,6 +1358,112 @@ static int ensure_backward_assets(dad3d_flame* h) {
   return DAD3D_OK;
 }
 
+// The stages of one backward pass of `rows` <= kDecodeChunk heads.  dad3d_flame_backward runs them in this order; the
+// dad3d_flame_backward_* test hooks run each one alone on caller buffers.
+// Forward blend product (recomputed): v_posed * basis_scale [rows, npad] fp32 from the prep kernel's coefficient rows
+static int bwd_blend_stage(dad3d_flame* h, const __half* a_hi, const __half* a_lo, int rows, float* vposed, cudaStream_t stream) {
+  GemmMaps maps;
+  const int rc = row_gemm_maps(&maps, a_hi, a_lo, rows, kKPad, kBlockM, h->map_b);
+  if (rc != DAD3D_OK) return rc;
+  const GemmGeom g = row_gemm_geom(rows, kKPad / kBlockK, h->n3, kBlendBlockN, 2);
+  EpiBlend::Params ep{vposed, h->npad};
+  return gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
+}
+
+// sigma's exponent cap: sigma <= 2^127 and sigma * basis_scale <= 2^127 (flame_bwd_gmax_kernel)
+static int sigma_emax(const dad3d_flame* h) {
+  int e;
+  std::frexp(h->basis_scale, &e);                   // basis_scale = 2^(e - 1)
+  return std::min(127, 127 - (e - 1));
+}
+
+// Per head sigma; D = dp * sigma * basis_scale as fp16 hi / lo rows [rows, npad] (padding columns zero); per 256-vertex block
+// the partial sums of the 30 transform cotangents
+static int bwd_vertex_stage(dad3d_flame* h, const float* vposed, const float* xf, const float* gv, const float* gp, int pc, int rows,
+                            float half_img, float* sigma, __half* d_hi, __half* d_lo, float* partial, cudaStream_t stream) {
+  flame_bwd_gmax_kernel<<<rows, 256, 0, stream>>>(gv, gp, pc, h->nv, xf, half_img, sigma_emax(h), sigma);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  DAD3D_CUDA_OK(cudaMemsetAsync(d_hi, 0, static_cast<size_t>(rows) * h->npad * sizeof(__half), stream));
+  DAD3D_CUDA_OK(cudaMemsetAsync(d_lo, 0, static_cast<size_t>(rows) * h->npad * sizeof(__half), stream));
+  dim3 grid(ceil_div(h->nv, 256), rows);
+  flame_bwd_vertex_kernel<<<grid, 256, 0, stream>>>(vposed, h->npad, h->d_w2, xf, gv, gp, pc, h->nv, half_img, sigma,
+                                                    h->basis_scale, d_hi, d_lo, partial);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+// The dense part: d coef [rows, 448] = D [rows, npad] x Basis_s [npad, 448]   (wgmma, fp16 hi/lo, 3 products)
+static int bwd_dense_stage(dad3d_flame* h, const __half* d_hi, const __half* d_lo, int rows, float* dcoef, cudaStream_t stream) {
+  GemmMaps maps;
+  const int rc = row_gemm_maps(&maps, d_hi, d_lo, rows, h->npad, kBlockM, h->map_bT);
+  if (rc != DAD3D_OK) return rc;
+  const GemmGeom g = row_gemm_geom(rows, h->npad / kBlockK, kKPad, 64, 2);
+  EpiBlend::Params ep{dcoef, kKPad};
+  return gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
+}
+
+// d coef and the cotangents -> the 413 parameter gradients of `rows` heads
+static int bwd_finalize_stage(dad3d_flame* h, const float* p, int rows, int flags, const float* dcoef, const float* partial,
+                              const float* sigma, float* gout, cudaStream_t stream) {
+  flame_bwd_finalize_kernel<<<ceil_div(rows * 32, 128), 128, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags,
+                                                                         1.0f / h->basis_scale, dcoef, partial,
+                                                                         ceil_div(h->nv, 256), sigma, h->basis_scale, gout);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+int dad3d_flame_backward_blend(dad3d_flame* h, const void* coef_hi_d, const void* coef_lo_d, int32_t B, float* vposed_d,
+                               dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && B <= kDecodeChunk, "B must fit one backward pass (1..4096 heads)");
+  DAD3D_REQUIRE(coef_hi_d && coef_lo_d && vposed_d, "null pointer");
+  DAD3D_REQUIRE(reinterpret_cast<uintptr_t>(vposed_d) % 16 == 0, "vposed_d must be 16-byte aligned (float4 stores)");
+  return bwd_blend_stage(h, static_cast<const __half*>(coef_hi_d), static_cast<const __half*>(coef_lo_d), B, vposed_d,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_flame_backward_vertex(dad3d_flame* h, const float* vposed_d, const float* xf_d, const float* grad_vertices_d,
+                                const float* grad_projected_d, int32_t B, float image_size, int32_t to_2d, float* sigma_d,
+                                void* d_hi_d, void* d_lo_d, float* partial_d, dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && B <= kDecodeChunk, "B must fit one backward pass (1..4096 heads)");
+  DAD3D_REQUIRE(vposed_d && xf_d && sigma_d && d_hi_d && d_lo_d && partial_d, "null pointer");
+  DAD3D_REQUIRE(grad_vertices_d || grad_projected_d, "at least one incoming gradient must be given");
+  return bwd_vertex_stage(h, vposed_d, xf_d, grad_vertices_d, grad_projected_d, to_2d ? 2 : 3, B, 0.5f * image_size, sigma_d,
+                          static_cast<__half*>(d_hi_d), static_cast<__half*>(d_lo_d), partial_d,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_flame_backward_dense(dad3d_flame* h, const void* d_hi_d, const void* d_lo_d, int32_t B, float* dcoef_d,
+                               dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && B <= kDecodeChunk, "B must fit one backward pass (1..4096 heads)");
+  DAD3D_REQUIRE(d_hi_d && d_lo_d && dcoef_d, "null pointer");
+  DAD3D_REQUIRE(reinterpret_cast<uintptr_t>(dcoef_d) % 16 == 0, "dcoef_d must be 16-byte aligned (float4 stores)");
+  DAD3D_REQUIRE(h->jaw_only, "backward is implemented for layouts without neck / eyeball pose (the released model)");
+  const int rc = ensure_backward_assets(h);
+  if (rc != DAD3D_OK) return rc;
+  return bwd_dense_stage(h, static_cast<const __half*>(d_hi_d), static_cast<const __half*>(d_lo_d), B, dcoef_d,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dad3d_flame_backward_finalize(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, const float* dcoef_d,
+                                  const float* partial_d, const float* sigma_d, float* grad_params_d, dad3d_stream stream) {
+  DAD3D_REQUIRE(h, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && B <= kDecodeChunk, "B must fit one backward pass (1..4096 heads)");
+  DAD3D_REQUIRE(params_d && dcoef_d && partial_d && sigma_d && grad_params_d, "null pointer");
+  DAD3D_REQUIRE(h->jaw_only, "backward is implemented for layouts without neck / eyeball pose (the released model)");
+  return bwd_finalize_stage(h, params_d, B, flags, dcoef_d, partial_d, sigma_d, grad_params_d,
+                            reinterpret_cast<cudaStream_t>(stream));
+}
+
 int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, const float* grad_vertices_d,
                          const float* grad_projected_d, float image_size, int32_t to_2d, float* grad_params_d,
                          void* workspace_d, size_t workspace_bytes, dad3d_stream stream_) {
@@ -1379,9 +1489,7 @@ int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32
   float* partial = reinterpret_cast<float*>(ws); ws += ws_partial_bytes(h, rows_max);
   float* sigma = reinterpret_cast<float*>(ws);
   const int pc = to_2d ? 2 : 3;
-  const float inv_scale = 1.0f / h->basis_scale;
   const float half_img = 0.5f * image_size;
-  const int n_blocks = ceil_div(h->nv, 256);
 
   for (int b0 = 0; b0 < B; b0 += chunk) {
     const int rows = (B - b0) < chunk ? (B - b0) : chunk;
@@ -1389,44 +1497,15 @@ int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_t B, int32
     const float* gv = grad_vertices_d ? grad_vertices_d + static_cast<size_t>(b0) * h->nv * 3 : nullptr;
     const float* gp = grad_projected_d ? grad_projected_d + static_cast<size_t>(b0) * h->nv * pc : nullptr;
     float* gout = grad_params_d + static_cast<size_t>(b0) * h->layout.n_params;
-    flame_prep_kernel<<<ceil_div(rows * 32, 256), 256, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags, inv_scale,
-                                                                     a_hi, a_lo, xf, 0, 1);
+    flame_prep_kernel<<<ceil_div(rows * 32, 256), 256, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags,
+                                                                     1.0f / h->basis_scale, a_hi, a_lo, xf, 0, 1);
     count_launch();
     DAD3D_CUDA_OK(cudaGetLastError());
-    {   // forward blend product (recomputed): v_posed * basis_scale -> scratch
-      GemmMaps maps;
-      rc = row_gemm_maps(&maps, a_hi, a_lo, rows, kKPad, kBlockM, h->map_b);
-      if (rc != DAD3D_OK) return rc;
-      const GemmGeom g = row_gemm_geom(rows, kKPad / kBlockK, h->n3, kBlendBlockN, 2);
-      EpiBlend::Params ep{vposed, h->npad};
-      rc = gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
-      if (rc != DAD3D_OK) return rc;
-    }
-    flame_bwd_gmax_kernel<<<rows, 256, 0, stream>>>(gv, gp, pc, h->nv, xf, half_img, sigma);
-    count_launch();
-    DAD3D_CUDA_OK(cudaGetLastError());
-    DAD3D_CUDA_OK(cudaMemsetAsync(d_hi, 0, static_cast<size_t>(rows) * h->npad * sizeof(__half), stream));
-    DAD3D_CUDA_OK(cudaMemsetAsync(d_lo, 0, static_cast<size_t>(rows) * h->npad * sizeof(__half), stream));
-    {
-      dim3 grid(n_blocks, rows);
-      flame_bwd_vertex_kernel<<<grid, 256, 0, stream>>>(vposed, h->npad, h->d_w2, xf, gv, gp, pc, h->nv, half_img, sigma,
-                                                        h->basis_scale, d_hi, d_lo, partial);
-      count_launch();
-      DAD3D_CUDA_OK(cudaGetLastError());
-    }
-    {   // the dense part: d coef [rows, 448] = D [rows, 15104] x Basis_s [15104, 448]   (wgmma, fp16 hi/lo, 3 products)
-      GemmMaps maps;
-      rc = row_gemm_maps(&maps, d_hi, d_lo, rows, h->npad, kBlockM, h->map_bT);
-      if (rc != DAD3D_OK) return rc;
-      const GemmGeom g = row_gemm_geom(rows, h->npad / kBlockK, kKPad, 64, 2);
-      EpiBlend::Params ep{dcoef, kKPad};
-      rc = gemm_launch<EpiBlend>(maps, g, ep, h->num_sms, &h->gemm_blend, false, stream);
-      if (rc != DAD3D_OK) return rc;
-    }
-    flame_bwd_finalize_kernel<<<ceil_div(rows * 32, 128), 128, 0, stream>>>(p, rows, h->layout, h->d_jt, h->d_jdirsT, flags, inv_scale,
-                                                                           dcoef, partial, n_blocks, sigma, h->basis_scale, gout);
-    count_launch();
-    DAD3D_CUDA_OK(cudaGetLastError());
+    if ((rc = bwd_blend_stage(h, a_hi, a_lo, rows, vposed, stream)) != DAD3D_OK) return rc;
+    if ((rc = bwd_vertex_stage(h, vposed, xf, gv, gp, pc, rows, half_img, sigma, d_hi, d_lo, partial, stream)) != DAD3D_OK)
+      return rc;
+    if ((rc = bwd_dense_stage(h, d_hi, d_lo, rows, dcoef, stream)) != DAD3D_OK) return rc;
+    if ((rc = bwd_finalize_stage(h, p, rows, flags, dcoef, partial, sigma, gout, stream)) != DAD3D_OK) return rc;
   }
   return DAD3D_OK;
 }

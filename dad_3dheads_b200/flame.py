@@ -238,6 +238,67 @@ class FlameDecoder:
                 projected.data_ptr() if projected is not None else None, float(image_size), 1 if to_2d else 0,
                 ws.data_ptr(), ws.numel(), torch.cuda.current_stream(params.device).cuda_stream), "dad3d_flame_decode")
 
+    # ---- test hooks: the stages of a backward pass on caller buffers (include/dad3d.h); B <= 4096 heads
+    def _npad(self) -> int:
+        return (3 * self.n_vertices + 127) // 128 * 128
+
+    def backward_blend(self, coef_hi: Tensor, coef_lo: Tensor, B: int, vposed: Tensor) -> None:
+        """The recomputed forward blend product: unpermuted prep rows -> ``vposed`` [B, npad] fp32 (v_posed * basis_scale)."""
+        for t in (coef_hi, coef_lo):
+            assert t.dtype == torch.float16 and t.is_contiguous() and t.shape[1] == 448 and t.shape[0] >= (B + 255) // 256 * 256
+        assert vposed.dtype == torch.float32 and vposed.is_contiguous() and vposed.shape == (B, self._npad())
+        with torch.cuda.device(vposed.device):
+            _lib.check(self.lib.dad3d_flame_backward_blend(self._h, coef_hi.data_ptr(), coef_lo.data_ptr(), int(B),
+                                                           vposed.data_ptr(),
+                                                           torch.cuda.current_stream(vposed.device).cuda_stream),
+                       "dad3d_flame_backward_blend")
+
+    def backward_vertex(self, vposed: Tensor, xf: Tensor, grad_vertices: Optional[Tensor], grad_projected: Optional[Tensor], *,
+                        sigma: Tensor, d_hi: Tensor, d_lo: Tensor, partial: Tensor, image_size: float = 256.0,
+                        to_2d: bool = True) -> None:
+        """Vertex stage: ``sigma`` [B], ``d_hi`` / ``d_lo`` [B, npad] fp16 and ``partial`` [B, ceil(V / 256), 32]."""
+        B, nv = xf.shape[0], self.n_vertices
+        assert vposed.dtype == torch.float32 and vposed.is_contiguous() and vposed.shape == (B, self._npad())
+        assert xf.dtype == torch.float32 and xf.is_contiguous() and xf.shape == (B, 68)
+        for t, shape in ((grad_vertices, (B, nv, 3)), (grad_projected, (B, nv, 2 if to_2d else 3))):
+            assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.shape == shape)
+        assert sigma.dtype == torch.float32 and sigma.is_contiguous() and sigma.shape == (B,)
+        for t in (d_hi, d_lo):
+            assert t.dtype == torch.float16 and t.is_contiguous() and t.shape == (B, self._npad())
+        assert partial.dtype == torch.float32 and partial.is_contiguous() and partial.shape == (B, (nv + 255) // 256, 32)
+        with torch.cuda.device(xf.device):
+            _lib.check(self.lib.dad3d_flame_backward_vertex(
+                self._h, vposed.data_ptr(), xf.data_ptr(), grad_vertices.data_ptr() if grad_vertices is not None else None,
+                grad_projected.data_ptr() if grad_projected is not None else None, B, float(image_size), 1 if to_2d else 0,
+                sigma.data_ptr(), d_hi.data_ptr(), d_lo.data_ptr(), partial.data_ptr(),
+                torch.cuda.current_stream(xf.device).cuda_stream), "dad3d_flame_backward_vertex")
+
+    def backward_dense(self, d_hi: Tensor, d_lo: Tensor, dcoef: Tensor) -> None:
+        """Dense stage: ``d_hi`` / ``d_lo`` [B, npad] fp16 -> ``dcoef`` [B, 448] fp32."""
+        B = dcoef.shape[0]
+        for t in (d_hi, d_lo):
+            assert t.dtype == torch.float16 and t.is_contiguous() and t.shape == (B, self._npad())
+        assert dcoef.dtype == torch.float32 and dcoef.is_contiguous() and dcoef.shape == (B, 448)
+        with torch.cuda.device(dcoef.device):
+            _lib.check(self.lib.dad3d_flame_backward_dense(self._h, d_hi.data_ptr(), d_lo.data_ptr(), B, dcoef.data_ptr(),
+                                                           torch.cuda.current_stream(dcoef.device).cuda_stream),
+                       "dad3d_flame_backward_dense")
+
+    def backward_finalize(self, params: Tensor, dcoef: Tensor, partial: Tensor, sigma: Tensor, grad_params: Tensor, *,
+                          flags: int = 0) -> None:
+        """Finalize stage: the parameter gradients [B, num_params] from ``dcoef``, ``partial`` and ``sigma``."""
+        B = params.shape[0]
+        assert params.dtype == torch.float32 and params.is_contiguous() and params.shape == (B, self.num_params)
+        assert dcoef.dtype == torch.float32 and dcoef.is_contiguous() and dcoef.shape == (B, 448)
+        assert partial.dtype == torch.float32 and partial.is_contiguous()
+        assert partial.shape == (B, (self.n_vertices + 255) // 256, 32)
+        assert sigma.dtype == torch.float32 and sigma.is_contiguous() and sigma.shape == (B,)
+        assert grad_params.dtype == torch.float32 and grad_params.is_contiguous() and grad_params.shape == params.shape
+        with torch.cuda.device(params.device):
+            _lib.check(self.lib.dad3d_flame_backward_finalize(
+                self._h, params.data_ptr(), B, int(flags), dcoef.data_ptr(), partial.data_ptr(), sigma.data_ptr(),
+                grad_params.data_ptr(), torch.cuda.current_stream(params.device).cuda_stream), "dad3d_flame_backward_finalize")
+
     def _check_out(self, t: Optional[Tensor], B: int, nc: int) -> None:
         if t is not None:
             assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == (B, self.n_vertices, nc), t.shape

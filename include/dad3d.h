@@ -120,6 +120,38 @@ DAD3D_API int dad3d_flame_backward(dad3d_flame* h, const float* params_d, int32_
                                    const float* grad_projected_d, float image_size, int32_t to_2d, float* grad_params_d,
                                    void* workspace_d, size_t workspace_bytes, dad3d_stream stream);
 
+/* test hooks: the stages of every backward pass, run alone on caller buffers.  dad3d_flame_backward runs each pass of up to
+ * 4096 heads as flame_prep_kernel (dad3d_flame_prep, permute = 0), then blend, vertex, dense and finalize below; each hook
+ * takes 1 <= B <= 4096 heads (else DAD3D_ERR_INVALID).  npad = dad3d_flame_describe's npad (3 V rounded up to 128).
+ *   dad3d_flame_backward_blend     the recomputed forward blend product: coef_hi_d / coef_lo_d [B rounded up to 256, 448] fp16
+ *                      unpermuted prep rows -> vposed_d [B, npad] fp32 = v_posed * basis_scale, x,y,z interleaved (columns
+ *                      3 V .. npad - 1 are written with the product of the zero basis rows); vposed_d 16-byte aligned
+ *   dad3d_flame_backward_vertex    vposed_d [B, npad] fp32, xf_d [B, 68] fp32 transform records (dad3d_flame_prep), the
+ *                      incoming gradients as in dad3d_flame_backward (either may be NULL, not both) ->
+ *                      sigma_d [B] fp32: the power of two that lifts the head's max |gV + (image/2) sc gP| into [512, 1024),
+ *                        its exponent capped so that sigma * basis_scale <= 2^127; 1 for an all-zero or non-finite maximum;
+ *                      d_hi_d / d_lo_d [B, npad] fp16: fp16 RN hi / lo split of dp * sigma * basis_scale, where
+ *                        dp = (w_rest A0'^T + w_jaw A2'^T) g per vertex coordinate; columns 3 V .. npad - 1 are zero;
+ *                      partial_d [B, ceil(V / 256), 32] fp32: per 256-vertex block, the block's sums of the cotangents
+ *                        G_A0'[9] g_t0[3] G_A2'[9] g_t2[3] g_c[3] d_sc d_tx d_ty (floats 30, 31 are not written)
+ *   dad3d_flame_backward_dense     d_hi_d / d_lo_d [B, npad] fp16 -> dcoef_d [B, 448] fp32 = (hi hi + (lo hi + hi lo)) over
+ *                      the transposed hi / lo basis planes (columns 0..399 betas, 400..435 pose features, the rest unused);
+ *                      dcoef_d 16-byte aligned (the epilogue stores float4)
+ *   dad3d_flame_backward_finalize  params_d [B, num_params], flags (DAD3D_ZERO_ROT / DAD3D_ZERO_JAW), dcoef_d, partial_d,
+ *                      sigma_d as above -> grad_params_d [B, num_params]: every entry of the released layout is written
+ *                      (translation z and the flagged entries as 0).  Non-finite incoming gradients may propagate to their
+ *                      own head's gradients; other heads are not affected. */
+DAD3D_API int dad3d_flame_backward_blend(dad3d_flame* h, const void* coef_hi_d, const void* coef_lo_d, int32_t B, float* vposed_d,
+                                         dad3d_stream stream);
+DAD3D_API int dad3d_flame_backward_vertex(dad3d_flame* h, const float* vposed_d, const float* xf_d, const float* grad_vertices_d,
+                                          const float* grad_projected_d, int32_t B, float image_size, int32_t to_2d,
+                                          float* sigma_d, void* d_hi_d, void* d_lo_d, float* partial_d, dad3d_stream stream);
+DAD3D_API int dad3d_flame_backward_dense(dad3d_flame* h, const void* d_hi_d, const void* d_lo_d, int32_t B, float* dcoef_d,
+                                         dad3d_stream stream);
+DAD3D_API int dad3d_flame_backward_finalize(dad3d_flame* h, const float* params_d, int32_t B, int32_t flags, const float* dcoef_d,
+                                            const float* partial_d, const float* sigma_d, float* grad_params_d,
+                                            dad3d_stream stream);
+
 DAD3D_API int dad3d_gather_landmarks(const float* src_d, int32_t B, int32_t n_vertices, int32_t ncomp, const int32_t* idx_d,
                            int32_t L, float* out_d, dad3d_stream stream);
 /* barycentric variant (model_training/data/utils.py:120-206 get_68_landmarks): out[b,l,:] = sum_k bary[l,k]*src[b,tri[l,k],:] */
