@@ -25,6 +25,8 @@ from . import _lib
 from .encoder import OUTPUT_2D_LANDMARKS, OUTPUT_3DMM_PARAMS, OUTPUT_LANDMARKS_HEATMAP, Dad3dEncoder
 from .flame import load_flame_static
 from .head_mesh import HeadMesh
+from . import overlay as overlay_ops
+from .overlay import OVERLAY_KINDS
 from .rasterizer import LitRenderer, PnccRenderer
 
 logger = logging.getLogger(__name__)
@@ -304,6 +306,26 @@ class FaceMeshPredictor:
             raise ValueError("frame_render needs to_2d=False: the renderer takes the projected vertices with their depth")
         return keys
 
+    @staticmethod
+    def _overlay_keys(overlay, boxes) -> Tuple[str, ...]:
+        """``overlay`` as a canonical tuple (the order of OVERLAY_KINDS), validated against ``boxes``."""
+        if overlay is None:
+            return ()
+        if isinstance(overlay, str):
+            overlay = (overlay,)
+        unknown = set(overlay) - set(OVERLAY_KINDS)
+        if unknown:
+            raise ValueError(f"overlay: unknown kinds {sorted(unknown)}; choose from {OVERLAY_KINDS}")
+        keys = tuple(k for k in OVERLAY_KINDS if k in overlay)
+        if keys and boxes is None:
+            raise ValueError("overlay needs boxes: it draws into copies of the frames, which the no-box path does not have")
+        return keys
+
+    def _rotation_index(self) -> int:
+        """Where FlameParams.from_3dmm (model/flame.py:41-101) reads the six rotation parameters."""
+        c = self.flame_constants
+        return c["shape"] + c["expression"] + c["jaw"]
+
     def _pncc_renderer(self) -> PnccRenderer:
         if self._renderer is None:                           # uploads its tables once (graph-capture safe afterwards)
             self._renderer = PnccRenderer(self.device)
@@ -340,7 +362,7 @@ class FaceMeshPredictor:
         return boxes, frame_index
 
     def _predict_rois(self, frames, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
-                      frame_render=()) -> Dict[str, Tensor]:
+                      frame_render=(), overlay=(), rpy=False) -> Dict[str, Tensor]:
         """predict_batch with boxes: crop geometry, pre-processing and read-back in csrc/roi.cu, no host synchronisation."""
         boxes, frame_index = self._check_rois(frames, boxes, frame_index)
         ext = np.array(extend_sides(extend), dtype=np.float64)
@@ -387,11 +409,26 @@ class FaceMeshPredictor:
                 out.update({f"frame_{k}": t for k, t in maps.items()})
             if "lit" in frame_render:
                 out["frame_lit"] = self._lit().render_frames(proj, frame_of_head, F, (H, W), frames=frames)["lit"]
+        if rpy or "pose" in overlay:
+            angles, pose = overlay_ops.pose_geometry(params, self._rotation_index(), rois if "pose" in overlay else None)
+            if rpy:
+                out["rpy"] = angles
+        if overlay:
+            copies = {k: frames.clone() for k in overlay}            # one device copy per kind, before any drawing
+            for k, img in copies.items():
+                if k == "68_landmarks":
+                    overlay_ops.draw_points(img, points, rois)
+                elif k == "pose":
+                    overlay_ops.draw_pose(img, pose)
+                else:                                                 # the demo's "445" draws every file: the 565 set
+                    subset = "191" if k == "191_landmarks" else "565"
+                    overlay_ops.draw_points(img, proj.contiguous(), rois, self._landmark_index(subset))
+                out[f"frame_{k}"] = img
         return out
 
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                       fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                      extend=0.0, frame_render=None) -> Dict[str, Tensor]:
+                      extend=0.0, frame_render=None, overlay=None, rpy: bool = False) -> Dict[str, Tensor]:
         """images: [B,3,256,256] fp32 already letter-boxed + normalised, or raw RGB as the reference's ``__call__`` takes it:
         one [B,H,W,3] uint8 tensor / a list of HxWx3 uint8 images (letter-boxed + normalised on the GPU, bit-identical to
         the reference's albumentations pipeline); host or device.  All outputs stay on the GPU:
@@ -427,14 +464,33 @@ class FaceMeshPredictor:
         ``PNCCEstimator()(frame, {"3dmm_params": p})`` run for its boxes' frame-space parameters one after the other in box
         order on the same buffers: the nearest head wins, an exact depth tie goes to the earlier box, invalid boxes draw
         nothing.  The reference's ``with_background=True`` overlay is, exactly,
-        ``torch.where(out["frame_head_index"][..., None] >= 0, out["frame_pncc"], frames)``."""
+        ``torch.where(out["frame_head_index"][..., None] >= 0, out["frame_pncc"], frames)``.
+
+        ``overlay`` (with ``boxes``): a subset of ("68_landmarks", "191_landmarks", "445_landmarks", "pose"), the demo's
+        ``type_of_output`` names.  Each adds "frame_<kind>" [F,H,W,3] uint8, a copy of the frames (never written) with that
+        overlay drawn by csrc/overlay.cu.  Frame f equals, byte for byte, a copy of frame f to which the reference's own
+        processor from ``demo_utils.py`` is applied for every valid box on it, in box order, with that box's predictions:
+        "68_landmarks" ``draw_landmarks({"points": points[r]}, copy)``; "191_landmarks" / "445_landmarks"
+        ``draw_3d_landmarks({"projected_vertices": projected_vertices[r]}, copy, subset)``, which truncates with
+        ``astype(int)`` and draws every file of the subset's directory -- so the demo's "445" draws the 565-point set
+        (``keypoints_565``), and "191" the 191 set; "pose" ``draw_pose({"3dmm_params": params[r:r+1]}, copy[y:y+h, x:x+w])``
+        into the crop view of ``crop_boxes[r]``: centre of the crop, arrow size h // 10, thickness int(h * 0.005), clipped at
+        the crop's border; later boxes, then later arrows (red, green, blue), win.  Where the reference has no defined
+        output, nothing is drawn: invalid boxes, points whose truncated coordinates are not finite or do not fit int32 (cv2
+        raises there), and the pose of a box whose crop is under 200 px high (thickness 0, which cv2.arrowedLine refuses;
+        its "rpy" is still written).  A whole image is the box [0, 0, W, H] with ``extend=0``.
+
+        ``rpy=True`` adds "rpy" [B|R,3] float64, (roll, pitch, yaw) in degrees: ``calculate_rpy`` on each head's parameters
+        (the reference computes head 0 only), to ~1e-12 degrees away from gimbal lock (scipy's SVD polar factor of the
+        fp32 rotation is taken by Newton steps on the device).  With boxes, the rotation is that of the crop: the read-back does not change it."""
         render = self._render_keys(render, to_2d)
         frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
+        overlay = self._overlay_keys(overlay, boxes)
         if boxes is not None:
             if render:
                 raise ValueError("render is not supported together with boxes")
             return self._predict_rois(images, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
-                                      frame_render)
+                                      frame_render, overlay, bool(rpy))
         if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
             x = self.preprocess_batch(images)
         else:
@@ -451,6 +507,8 @@ class FaceMeshPredictor:
                                       tri_index="tri_index" in render))
         if "lit" in render:
             out.update(self._lit()(proj, self._img_size))
+        if rpy:
+            out["rpy"] = overlay_ops.pose_geometry(params, self._rotation_index())[0]
         return out
 
     def _ws_generation(self):
@@ -458,11 +516,14 @@ class FaceMeshPredictor:
         dec = self.head_mesh.flame.decoder(self.device)
         return (self.model.ws_generation, dec.ws_generation)
 
-    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None, frame_render=()):
+    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None, frame_render=(),
+                 overlay=(), rpy=False):
         """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph.
         ``rois`` = (static boxes [R,4] int32, static frame index [R] int32, extend): the graph reads the boxes from those
         buffers on every replay."""
-        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2], frame_render=frame_render) if rois is not None else {}
+        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2], frame_render=frame_render,
+                  overlay=overlay) if rois is not None else {}
+        kw["rpy"] = rpy
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
@@ -490,7 +551,7 @@ class FaceMeshPredictor:
 
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                               fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                              extend=0.0, frame_render=None) -> Dict[str, Tensor]:
+                              extend=0.0, frame_render=None, overlay=None, rpy: bool = False) -> Dict[str, Tensor]:
         """:meth:`predict_batch` replayed from a CUDA graph (one graph per input shape / dtype / option set): the ~110 kernel
         launches of a step become one graph launch, which removes the launch gaps between the many sub-20 us layers.
         ``images`` is copied into the graph's static input buffer (host or device source); the returned tensors are the
@@ -501,11 +562,13 @@ class FaceMeshPredictor:
         re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced.
 
         With ``boxes`` (see :meth:`predict_batch`) the boxes and frame indices are copied into static buffers as well: one
-        graph serves every box set of the same frame shape, box count, ``extend`` and ``frame_render``."""
+        graph serves every box set of the same frame shape, box count, ``extend``, ``frame_render`` and ``overlay``."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
         render = self._render_keys(render, to_2d)
         frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
-        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render, frame_render)
+        overlay = self._overlay_keys(overlay, boxes)
+        rpy = bool(rpy)
+        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy)
         if boxes is not None:
             if render:
                 raise ValueError("render is not supported together with boxes")
@@ -521,7 +584,8 @@ class FaceMeshPredictor:
             rois = self._roi_buffers(int(boxes.shape[0]), extend) if boxes is not None else None
             if rois is not None:
                 self._fill_rois(rois, boxes, frame_index)
-            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois, frame_render)
+            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois, frame_render,
+                                            overlay, rpy)
             ent = (graph, static_in, out, gen, rois)
             self._graphs[key] = ent
         graph, static_in, out, _, rois = ent
@@ -533,8 +597,8 @@ class FaceMeshPredictor:
 
     def open_stream(self, shape, dtype=torch.uint8, **kw) -> "BatchStream":
         """A double-buffered pipeline over :meth:`predict_batch` for a fixed batch signature -- see :class:`BatchStream`.
-        ``rois=R`` (with optional ``extend`` and ``frame_render``): ``shape`` is that of the frames, and every submit brings R
-        boxes."""
+        ``rois=R`` (with optional ``extend``, ``frame_render`` and ``overlay``): ``shape`` is that of the frames, and every submit
+        brings R boxes.  ``rpy`` is passed to ``predict_batch``."""
         return BatchStream(self, shape, dtype, **kw)
 
 
@@ -550,14 +614,14 @@ class BatchStream:
     ``keys`` to have them copied to the host like the other outputs.  With ``rois=R`` each batch is frames plus R boxes
     (``predict_batch``'s ``boxes``): ``submit(frames, boxes=, frame_index=)`` copies the boxes on the copy stream together with
     the frames; "crop_boxes" and "valid" may be listed in ``keys``, and with ``frame_render`` (passed to ``predict_batch``)
-    the "frame_<map>" outputs too.
+    the "frame_<map>" outputs too; likewise "frame_<kind>" with ``overlay`` and "rpy" with ``rpy=True``.
     """
 
     def __init__(self, predictor: FaceMeshPredictor, shape, dtype=torch.uint8, landmark_subset: Optional[str] = "445",
                  to_2d: bool = True, fast_decode: bool = True, depth: int = 2, render=None,
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
                  group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None, rois=None,
-                 extend=0.0, frame_render=None):
+                 extend=0.0, frame_render=None, overlay=None, rpy: bool = False):
         self.pred = predictor
         dev = predictor.device
         self.device = dev
@@ -575,13 +639,16 @@ class BatchStream:
         if rois is not None and self._args[3]:
             raise ValueError("render is not supported together with boxes")
         self._frame_render = predictor._frame_render_keys(frame_render, to_2d, rois)
+        self._overlay = predictor._overlay_keys(overlay, rois)
+        self._rpy = bool(rpy)
         self.rois = rois
         self.slots = []
         with torch.cuda.device(dev):
             for _ in range(self.depth):
                 static_in = torch.zeros(tuple(shape), dtype=dtype, device=dev)
                 roi_bufs = predictor._roi_buffers(int(rois), extend) if rois is not None else None
-                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs, self._frame_render)
+                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs, self._frame_render, self._overlay,
+                                                     self._rpy)
                 slot = {"in": static_in, "rois": roi_bufs, "graph": graph, "out": out, "gen": gen, "busy": False,
                         "h2d": torch.cuda.Event(), "done": torch.cuda.Event(), "comm_done": torch.cuda.Event(),
                         "d2h": torch.cuda.Event(), "gathered": {}, "host": {}}
@@ -613,7 +680,8 @@ class BatchStream:
         s = self.slots[self._head]
         if s["gen"] != self.pred._ws_generation():           # scratch reallocated by another caller: re-capture this slot
             torch.cuda.synchronize(self.device)
-            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"], self._frame_render)
+            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"], self._frame_render,
+                                                                self._overlay, self._rpy)
         with torch.cuda.stream(self.copy_in):
             self.copy_in.wait_event(s["done"])               # the previous replay of this slot has consumed its input
             s["in"].copy_(images, non_blocking=True)

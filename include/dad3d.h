@@ -401,6 +401,43 @@ DAD3D_API int dad3d_render_lit(const float* vertices_d, int32_t nv, int32_t batc
                                dad3d_lighting lighting, const int32_t* image_of_head_d, int32_t n_images, int32_t h, int32_t w,
                                float* light_ws_d, uint8_t* image_d, unsigned long long* key_ws_d, dad3d_stream stream);
 
+/* ---- overlays: the demo's landmark and pose drawings, and head pose angles ----------------------------------------------
+ * Draws what demo_utils.py's processors draw with cv2 (4.13.0; the rules are restated and pinned in tests/overlay_model.py),
+ * byte for byte, into frames the caller has already copied, for R boxes at once, with every box-dependent value read on
+ * the device from the dad3d_roi records (see "heads from boxes").  Invalid records draw nothing.
+ *   dad3d_pose_geometry  replaces calculate_rpy (model_training/model/flame.py:238-264) for every head, and draw_pose's
+ *     float-to-integer geometry (demo_utils.py:68-94).  params_d [R,num_params] fp32; the six rotation parameters start at
+ *     rotation_index.  rot_mat_from_6dof (model/utils.py:92-101) in fp32 in torch's CPU operation order (bit-exact; rot_d
+ *     [R,3,3] fp32 receives it when not NULL), then scipy 1.18's Rotation.from_matrix(R^T) in fp64 -- the orthogonal polar
+ *     factor that scipy takes by SVD, here by three Newton steps (within ~1e-15 of it), then the quaternion -- and
+ *     as_euler("xyz", degrees=True), then limit_angle -> rpy_d [R,3] fp64 (roll, pitch, yaw; may be NULL).  With rois_d, pose_d [R,32] int32 records:
+ *     [draw, frame, x, y, w, h, thickness, 0, cx, cy, then per arrow (red, green, blue): end x, end y, tip1 x, tip1 y,
+ *     tip2 x, tip2 y, then zeros], in the coordinates of the crop view frame[y:y+h, x:x+w] that draw_pose is given: centre
+ *     (w // 2, h // 2), size h // 10, thickness int(h * 0.005), ends truncated, tips cvRound of cv2.arrowedLine's fp64
+ *     expressions.  draw = 0 for an invalid record, a crop under 200 px high (thickness 0: cv2.arrowedLine refuses it) or
+ *     non-finite angles.  rois_d and pose_d are both given or both NULL.  One thread per head.
+ *   dad3d_overlay_points  replaces draw_points over draw_landmarks / draw_3d_landmarks (demo_utils.py:22-47): for every
+ *     valid record r and l < L, the filled circle (radius, colour color_h[3] RGB bytes) at point index_d[l] (NULL: l) of
+ *     head r in points_d [R,n_src,ncomp] (is_float = 0: int64; 1: fp32 truncated toward zero, as astype(int)), drawn into
+ *     frames_d [F,H,W,3] frame rois_d[r].frame.  A point that is not finite or whose integers do not fit int32 draws nothing
+ *     (cv2 raises there), as does an index outside [0, n_src).  Every write of a call is the same colour, so the order of
+ *     the threads does not matter.
+ *   dad3d_overlay_pose  replaces draw_pose's three cv2.arrowedLine calls (demo_utils.py:90-92) for every record of
+ *     dad3d_pose_geometry, each clipped to its own crop view and to the frame (records from dad3d_roi records of the same
+ *     F, H, W always lie inside it): clears key_ws_d [F,H,W] int32, marks every covered pixel with
+ *     the largest 3 * box + arrow + 1 (the reference's last writer: box order, then red, green, blue), then writes the
+ *     winning arrow's colour over frames_d.  R <= (2^31 - 4) / 3. */
+#define DAD3D_POSE_RECORD_INTS 32
+DAD3D_API int dad3d_pose_geometry(const float* params_d, int32_t R, int32_t num_params, int32_t rotation_index,
+                                  const dad3d_roi* rois_d, double* rpy_d, int32_t* pose_d, float* rot_d,
+                                  dad3d_stream stream);
+DAD3D_API int dad3d_overlay_points(const void* points_d, int32_t is_float, int32_t R, int32_t n_src, int32_t ncomp,
+                                   const int64_t* index_d, int32_t L, const dad3d_roi* rois_d, int32_t radius,
+                                   const uint8_t* color_h, uint8_t* frames_d, int32_t F, int32_t H, int32_t W,
+                                   dad3d_stream stream);
+DAD3D_API int dad3d_overlay_pose(const int32_t* pose_d, int32_t R, int32_t* key_ws_d, uint8_t* frames_d, int32_t F,
+                                 int32_t H, int32_t W, dad3d_stream stream);
+
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
 
