@@ -105,6 +105,8 @@ SIGNATURES = {
                                         C.c_void_p]),
     "dad3d_overlay_pose": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_void_p]),
+    "dad3d_overlay_mesh": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "dad3d_comm_unique_id": (C.c_int, [C.c_void_p]),
     "dad3d_comm_init": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "dad3d_comm_destroy": (None, [C.c_void_p]),

@@ -1,12 +1,13 @@
-// The demo's landmark and pose overlays drawn into whole frames (include/dad3d.h "overlays"): draw_points over
-// draw_landmarks / draw_3d_landmarks (demo_utils.py:22-47), draw_pose (demo_utils.py:68-94) into each box's crop view, and
-// calculate_rpy (model_training/model/flame.py:238-264) for every head.
+// The demo's landmark, pose and wireframe overlays drawn into whole frames (include/dad3d.h "overlays"): draw_points over
+// draw_landmarks / draw_3d_landmarks (demo_utils.py:22-47), draw_pose (demo_utils.py:68-94) into each box's crop view,
+// draw_mesh (demo_utils.py:50-65), and calculate_rpy (model_training/model/flame.py:238-264) for every head.
 //
 // The raster restates the cv2 calls the demo makes (cv2 4.13.0; tests/overlay_model.py is the model, pinned against the
-// binary): the midpoint filled circle, the clipped 8-connected line iterator, and for thickness >= 2 the segment clipped to
-// the area grown by the thickness, a 16-bit fixed-point quad (outline by the fixed-point line, inside by the convex
-// scan-line fill) and two cap circles.  All of it is integer work in cv2's own int64 / double expressions; fp64 values use
+// binary; tests/wireframe_model.py for LineAA): the midpoint filled circle, the clipped 8-connected line iterator, the
+// anti-aliased line, and for thickness >= 2 the segment clipped to the area grown by the thickness, a 16-bit fixed-point
+// quad (outline by the fixed-point line, inside by the convex scan-line fill) and two cap circles.  All of it is integer work in cv2's own int64 / double expressions; fp64 values use
 // explicit _rn intrinsics so nvcc cannot contract them into an fma.
+#include <climits>
 #include <cstdint>
 
 #include "../../include/dad3d.h"
@@ -551,8 +552,286 @@ __global__ void pose_resolve_kernel(const int* __restrict__ key, size_t n, uint8
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------- wireframes
+// draw_mesh (demo_utils.py:50-65): cv2.line(img, p, q, EDGE_COLOR, 1, LINE_AA) per edge in order, i.e. cv2's LineAA.  Its
+// blends do not commute, so every pixel must see its (box, edge) stamps in order.  A tile CTA owns its pixels in registers
+// and walks the boxes, then each box's edges in chunks of blockDim, in order; a walk stamps a pixel at most once, so each
+// pixel folds its stamps in exactly cv2's order.  No fragment arena: memory is [R, 5] ints whatever the heads look like.
+
+constexpr int kMeshTile = 32;                          // tile side in pixels
+constexpr int kMeshThreads = 256;
+constexpr int kMeshPix = kMeshTile * kMeshTile / kMeshThreads;
+constexpr int kMeshMargin = 3;                         // covers the 3-pixel stamp and the step one past the second end
+constexpr int kMeshWsInts = DAD3D_MESH_WS_INTS;
+
+__constant__ int c_slope_corr[32] = {181, 181, 181, 182, 182, 183, 184, 185, 187, 188, 190, 192, 194, 196, 198, 201,
+                                     203, 206, 209, 211, 214, 218, 221, 224, 227, 231, 235, 238, 242, 246, 250, 254};
+__constant__ int c_filter[64] = {168, 177, 185, 194, 202, 210, 218, 224, 231, 236, 241, 246, 249, 252, 254, 254,
+                                 254, 254, 252, 249, 246, 241, 236, 231, 224, 218, 210, 202, 194, 185, 177, 168,
+                                 158, 149, 140, 131, 122, 114, 105, 97,  89,  82,  75,  68,  62,  56,  50,  45,
+                                 40,  36,  32,  28,  25,  22,  19,  16,  14,  12,  11,  9,   8,   7,   5,   5};
+
+// One LineAA walk: step k = 0..count visits major coordinate m0 + k at minor position minor0 + k * step (16.16).
+struct MeshWalk {
+  long long minor0, step;
+  int m0, count;
+  uint16_t ep[9];                                      // the end-point table, indexed min(k, 2) * 3 + min(count - k, 2)
+  uint8_t x_major;
+};
+
+// LineAA's set-up (drawing.cpp) for integer end points in a w x h image; false when clipLine leaves nothing.
+__device__ bool line_aa_walk(long long x1, long long y1, long long x2, long long y2, long long w, long long h,
+                             MeshWalk& o) {
+  x1 *= kXYOne; y1 *= kXYOne; x2 *= kXYOne; y2 *= kXYOne;
+  if (!clip_line(w << kXYShift, h << kXYShift, x1, y1, x2, y2)) return false;
+  long long dx = x2 - x1, dy = y2 - y1;
+  const long long j = dx < 0 ? -1 : 0, ax = (dx ^ j) - j;
+  const long long i = dy < 0 ? -1 : 0, ay = (dy ^ i) - i;
+  long long e1, e2;
+  o.x_major = ax > ay;
+  if (o.x_major) {
+    dy = (dy ^ j) - j;
+    if (j) {
+      long long t = x1; x1 = x2; x2 = t;
+      t = y1; y1 = y2; y2 = t;
+    }
+    o.step = (dy * kXYOne) / (ax | 1);
+    x2 += kXYOne;
+    o.count = static_cast<int>((x2 >> kXYShift) - (x1 >> kXYShift));
+    y1 += ((o.step * -(x1 & (kXYOne - 1))) >> kXYShift) + (kXYOne >> 1);
+    o.m0 = static_cast<int>(x1 >> kXYShift);
+    o.minor0 = y1;
+    e1 = x1; e2 = x2;
+  } else {
+    dx = (dx ^ i) - i;
+    if (i) {
+      long long t = x1; x1 = x2; x2 = t;
+      t = y1; y1 = y2; y2 = t;
+    }
+    o.step = (dx * kXYOne) / (ay | 1);
+    y2 += kXYOne;
+    o.count = static_cast<int>((y2 >> kXYShift) - (y1 >> kXYShift));
+    x1 += ((o.step * -(y1 & (kXYOne - 1))) >> kXYShift) + (kXYOne >> 1);
+    o.m0 = static_cast<int>(y1 >> kXYShift);
+    o.minor0 = x1;
+    e1 = y1; e2 = y2;
+  }
+  int slope = static_cast<int>((o.step >> (kXYShift - 5)) & 0x3f);
+  slope ^= o.step < 0 ? 0x3f : 0;
+  slope = (slope & 0x20) ? 0x100 : c_slope_corr[slope];
+  const int fi = static_cast<int>((e1 >> (kXYShift - 7)) & 0x78), fj = static_cast<int>((e2 >> (kXYShift - 7)) & 0x78);
+  const int t0 = slope << 7, t1 = ((0x78 - fi) | 4) * slope, t2 = (fj | 4) * slope;
+  o.ep[0] = 0;
+  o.ep[8] = static_cast<uint16_t>(slope);
+  o.ep[1] = o.ep[3] = static_cast<uint16_t>(((((fj - fi) & 0x78) | 4) * slope >> 8) & 0x1ff);
+  o.ep[2] = static_cast<uint16_t>((t1 >> 8) & 0x1ff);
+  o.ep[4] = static_cast<uint16_t>(((((fj - fi) + 0x80) | 4) * slope >> 8) & 0x1ff);
+  o.ep[5] = static_cast<uint16_t>(((t1 + t0) >> 8) & 0x1ff);
+  o.ep[6] = static_cast<uint16_t>((t2 >> 8) & 0x1ff);
+  o.ep[7] = static_cast<uint16_t>(((t2 + t0) >> 8) & 0x1ff);
+  return true;
+}
+
+// Per-box pass, one CTA per box: ws[r] = (frame if the box draws, else -1; then the pixel box x0, y0, x1, y1 that its
+// stamps can touch, clipped to the frame).  A box draws when its record is valid and every end point of every edge is
+// finite and fits int32 after truncation (cv2 raises otherwise, and draw_mesh has no output) -- and it touches the frame.
+__global__ void mesh_box_kernel(const float* __restrict__ verts, int nv, int ncomp, const int32_t* __restrict__ edges,
+                                int E, const dad3d_roi* __restrict__ rois, int F, int H, int W, int32_t* __restrict__ ws) {
+  const int r = blockIdx.x;
+  __shared__ long long s_box[4];
+  if (threadIdx.x == 0) {
+    s_box[0] = s_box[1] = LLONG_MAX;
+    s_box[2] = s_box[3] = LLONG_MIN;
+  }
+  __syncthreads();
+  long long x0 = LLONG_MAX, y0 = LLONG_MAX, x1 = LLONG_MIN, y1 = LLONG_MIN;
+  bool ok = true;
+  const float* v = verts + static_cast<size_t>(r) * nv * ncomp;
+  for (int e = threadIdx.x; e < 2 * E && ok; e += blockDim.x) {
+    const int idx = edges[e];
+    long long x, y;
+    if (idx < 0 || idx >= nv || !to_int32(static_cast<double>(v[static_cast<size_t>(idx) * ncomp]), x) ||
+        !to_int32(static_cast<double>(v[static_cast<size_t>(idx) * ncomp + 1]), y)) {
+      ok = false;
+      break;
+    }
+    x0 = min(x0, x); x1 = max(x1, x);
+    y0 = min(y0, y); y1 = max(y1, y);
+  }
+  const bool all_ok = __syncthreads_and(ok);
+  if (x0 <= x1) {
+    atomicMin(&s_box[0], x0); atomicMin(&s_box[1], y0);
+    atomicMax(&s_box[2], x1); atomicMax(&s_box[3], y1);
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  const dad3d_roi q = rois[r];
+  const long long bx0 = max(s_box[0] - kMeshMargin, 0LL), by0 = max(s_box[1] - kMeshMargin, 0LL);
+  const long long bx1 = min(s_box[2] + kMeshMargin, W - 1LL), by1 = min(s_box[3] + kMeshMargin, H - 1LL);
+  const bool draw = q.valid && q.frame >= 0 && q.frame < F && all_ok && E > 0 && bx0 <= bx1 && by0 <= by1;
+  int32_t* o = ws + static_cast<size_t>(r) * kMeshWsInts;
+  o[0] = draw ? q.frame : -1;
+  o[1] = draw ? static_cast<int32_t>(bx0) : 0;
+  o[2] = draw ? static_cast<int32_t>(by0) : 0;
+  o[3] = draw ? static_cast<int32_t>(bx1) : -1;
+  o[4] = draw ? static_cast<int32_t>(by1) : -1;
+}
+
+// Exclusive position of this thread's flag among the block's set flags, in thread order; *total = their count.
+__device__ __forceinline__ int block_compact(bool flag, int* s_warp, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned m = __ballot_sync(0xffffffffu, flag);
+  if (lane == 0) s_warp[warp] = __popc(m);
+  __syncthreads();
+  int base = 0, n = 0;
+  for (int k = 0; k < kMeshThreads / 32; ++k) {
+    base += k < warp ? s_warp[k] : 0;
+    n += s_warp[k];
+  }
+  *total = n;
+  return base + __popc(m & ((1u << lane) - 1u));
+}
+
+// Tile pass: one CTA per (frame, kMeshTile^2 tile); each thread holds kMeshPix pixels of it in registers.
+__global__ void __launch_bounds__(kMeshThreads) mesh_tile_kernel(
+    const float* __restrict__ verts, int nv, int ncomp, const int32_t* __restrict__ edges, int E, int R,
+    const int32_t* __restrict__ ws, int c0, int c1, int c2, uint8_t* __restrict__ frames, int H, int W, int tiles_x,
+    int tiles_y) {
+  __shared__ MeshWalk s_walk[kMeshThreads];
+  __shared__ int s_box[kMeshThreads];
+  __shared__ int s_warp[kMeshThreads / 32];
+  __shared__ int s_filter[64];
+  if (threadIdx.x < 64) s_filter[threadIdx.x] = c_filter[threadIdx.x];
+  const long long t = blockIdx.x;
+  const int f = static_cast<int>(t / (static_cast<long long>(tiles_x) * tiles_y));
+  const int rem = static_cast<int>(t % (static_cast<long long>(tiles_x) * tiles_y));
+  const int tx0 = (rem % tiles_x) * kMeshTile, ty0 = (rem / tiles_x) * kMeshTile;
+  const int tx1 = min(tx0 + kMeshTile, W) - 1, ty1 = min(ty0 + kMeshTile, H) - 1;
+  uint8_t* img = frames + static_cast<size_t>(f) * H * W * 3;
+  int px[kMeshPix], py[kMeshPix], col[kMeshPix][3];
+#pragma unroll
+  for (int p = 0; p < kMeshPix; ++p) {
+    const int l = threadIdx.x + p * kMeshThreads;
+    px[p] = tx0 + l % kMeshTile;
+    py[p] = ty0 + l / kMeshTile;
+    if (px[p] <= tx1 && py[p] <= ty1) {
+      const uint8_t* q = img + (static_cast<size_t>(py[p]) * W + px[p]) * 3;
+      col[p][0] = q[0]; col[p][1] = q[1]; col[p][2] = q[2];
+    } else {
+      px[p] = -1;                                      // outside the frame: cv2 never stamps it
+    }
+  }
+  bool dirty = false;
+  for (int rb = 0; rb < R; rb += kMeshThreads) {       // the boxes that touch this tile, in order
+    const int r = rb + threadIdx.x;
+    bool hit = false;
+    if (r < R) {
+      const int32_t* b = ws + static_cast<size_t>(r) * kMeshWsInts;
+      hit = b[0] == f && b[1] <= tx1 && b[3] >= tx0 && b[2] <= ty1 && b[4] >= ty0;
+    }
+    int nbox;
+    const int pos = block_compact(hit, s_warp, &nbox);
+    if (hit) s_box[pos] = r;
+    __syncthreads();
+    for (int bi = 0; bi < nbox; ++bi) {
+      const float* v = verts + static_cast<size_t>(s_box[bi]) * nv * ncomp;
+      for (int eb = 0; eb < E; eb += kMeshThreads) {   // the box's edges that touch the tile, in order
+        const int e = eb + threadIdx.x;
+        bool keep = false;
+        MeshWalk wk;
+        if (e < E) {
+          const int a = edges[2 * static_cast<size_t>(e)], b = edges[2 * static_cast<size_t>(e) + 1];
+          // the box draws, so both ends are finite and fit int32
+          const long long ax = __float2ll_rz(v[static_cast<size_t>(a) * ncomp]);
+          const long long ay = __float2ll_rz(v[static_cast<size_t>(a) * ncomp + 1]);
+          const long long bx = __float2ll_rz(v[static_cast<size_t>(b) * ncomp]);
+          const long long by = __float2ll_rz(v[static_cast<size_t>(b) * ncomp + 1]);
+          keep = min(ax, bx) - kMeshMargin <= tx1 && max(ax, bx) + kMeshMargin >= tx0 &&
+                 min(ay, by) - kMeshMargin <= ty1 && max(ay, by) + kMeshMargin >= ty0 &&
+                 line_aa_walk(ax, ay, bx, by, W, H, wk);
+          if (keep) {                                  // the steps inside the tile's major range touch its minor range?
+            const int lo = wk.x_major ? tx0 : ty0, hi = wk.x_major ? tx1 : ty1;
+            const int mlo = wk.x_major ? ty0 : tx0, mhi = wk.x_major ? ty1 : tx1;
+            const long long k0 = max(0LL, static_cast<long long>(lo) - wk.m0);
+            const long long k1 = min(static_cast<long long>(wk.count), static_cast<long long>(hi) - wk.m0);
+            if (k0 > k1) {
+              keep = false;
+            } else {
+              const long long ya = (wk.minor0 + k0 * wk.step) >> kXYShift, yb = (wk.minor0 + k1 * wk.step) >> kXYShift;
+              keep = min(ya, yb) - 1 <= mhi && max(ya, yb) + 1 >= mlo;
+            }
+          }
+        }
+        int n;
+        const int wpos = block_compact(keep, s_warp, &n);
+        if (keep) s_walk[wpos] = wk;
+        __syncthreads();
+        for (int q = 0; q < n; ++q) {
+          const MeshWalk& w = s_walk[q];
+#pragma unroll
+          for (int p = 0; p < kMeshPix; ++p) {
+            if (px[p] < 0) continue;
+            const long long k = static_cast<long long>(w.x_major ? px[p] : py[p]) - w.m0;
+            if (k < 0 || k > w.count) continue;
+            const long long y = w.minor0 + k * w.step;
+            const int o = (w.x_major ? py[p] : px[p]) - (static_cast<int>(y >> kXYShift) - 1);
+            if (o < 0 || o > 2) continue;
+            const int dist = static_cast<int>((y >> (kXYShift - 5)) & 31);
+            const int fidx = o == 0 ? dist + 32 : (o == 1 ? dist : 63 - dist);
+            const int ei = static_cast<int>(min(k, 2LL) * 3 + min(static_cast<long long>(w.count) - k, 2LL));
+            const int al = (w.ep[ei] * s_filter[fidx] >> 8) & 0xff;
+            const int cc[3] = {c0, c1, c2};
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) {           // cv2 applies the blend twice
+              int x = col[p][ch];
+              x += ((cc[ch] - x) * al + 127) >> 8;
+              x += ((cc[ch] - x) * al + 127) >> 8;
+              col[p][ch] = x;
+            }
+            dirty = true;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    __syncthreads();
+  }
+  if (!dirty) return;
+#pragma unroll
+  for (int p = 0; p < kMeshPix; ++p) {
+    if (px[p] < 0) continue;
+    uint8_t* q = img + (static_cast<size_t>(py[p]) * W + px[p]) * 3;
+    q[0] = static_cast<uint8_t>(col[p][0]);
+    q[1] = static_cast<uint8_t>(col[p][1]);
+    q[2] = static_cast<uint8_t>(col[p][2]);
+  }
+}
+
 }  // namespace
 }  // namespace dad3d
+
+extern "C" int dad3d_overlay_mesh(const float* vertices_d, int32_t R, int32_t nv, int32_t ncomp, const int32_t* edges_d,
+                                  int32_t E, const dad3d_roi* rois_d, const uint8_t* color_h, int32_t* ws_d,
+                                  uint8_t* frames_d, int32_t F, int32_t H, int32_t W, dad3d_stream stream) {
+  using namespace dad3d;
+  DAD3D_REQUIRE(R >= 0 && E >= 0, "R, E");
+  if (R == 0 || E == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(vertices_d && edges_d && rois_d && color_h && ws_d && frames_d, "null pointer");
+  DAD3D_REQUIRE(nv > 0 && (ncomp == 2 || ncomp == 3) && F > 0 && H > 0 && W > 0 && E <= INT32_MAX / 2, "sizes");
+  const long long tiles_x = (W + kMeshTile - 1) / kMeshTile, tiles_y = (H + kMeshTile - 1) / kMeshTile;
+  const long long tiles = tiles_x * tiles_y * F;
+  DAD3D_REQUIRE(tiles <= INT32_MAX, "too many tiles");
+  auto s = reinterpret_cast<cudaStream_t>(stream);
+  mesh_box_kernel<<<R, 256, 0, s>>>(vertices_d, nv, ncomp, edges_d, E, rois_d, F, H, W, ws_d);
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  mesh_tile_kernel<<<static_cast<unsigned>(tiles), kMeshThreads, 0, s>>>(
+      vertices_d, nv, ncomp, edges_d, E, R, ws_d, color_h[0], color_h[1], color_h[2], frames_d, H, W,
+      static_cast<int>(tiles_x), static_cast<int>(tiles_y));
+  count_launch();
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
 
 extern "C" int dad3d_pose_geometry(const float* params_d, int32_t R, int32_t num_params, int32_t rotation_index,
                                    const dad3d_roi* rois_d, double* rpy_d, int32_t* pose_d, float* rot_d,

@@ -1,11 +1,13 @@
-"""The demo's landmark and pose overlays drawn into whole frames on the GPU (csrc/overlay.cu), and head pose angles.
+"""The demo's landmark, pose and wireframe overlays drawn into whole frames on the GPU (csrc/overlay.cu), and head pose
+angles.
 
-``demo.py``'s ``68_landmarks``, ``191_landmarks``, ``445_landmarks`` and ``pose`` outputs are cv2 drawings made by
-``demo_utils.py`` (``draw_landmarks``, ``draw_3d_landmarks``, ``draw_pose``, lines 22-94), one image at a time on the host.
+``demo.py``'s ``68_landmarks``, ``191_landmarks``, ``445_landmarks``, ``pose``, ``head_mesh`` and ``face_mesh`` outputs are
+cv2 drawings made by ``demo_utils.py`` (``draw_landmarks``, ``draw_3d_landmarks``, ``draw_mesh``, ``draw_pose``, lines
+22-94), one image at a time on the host.
 These functions draw the same pixels, byte for byte, for every box of a batch of frames, from device tensors and without a
 host synchronisation, so they run inside a captured CUDA graph.  ``rpy`` is ``calculate_rpy``
 (model_training/model/flame.py:254-259) for every head instead of head 0.  The drawing rules (cv2 4.13.0) are restated in
-``tests/overlay_model.py``; DESIGN §4.8 lists them and what draws nothing.
+``tests/overlay_model.py`` and ``tests/wireframe_model.py``; DESIGN §4.8 lists them and what draws nothing.
 """
 from __future__ import annotations
 
@@ -17,10 +19,23 @@ from torch import Tensor
 
 from . import _lib
 
-OVERLAY_KINDS = ("68_landmarks", "191_landmarks", "445_landmarks", "pose")
+OVERLAY_KINDS = ("68_landmarks", "191_landmarks", "445_landmarks", "pose", "head_mesh", "face_mesh")
 POINT_COLOR = (255, 0, 0)                  # demo_utils.POINT_COLOR
+EDGE_COLOR = (39, 48, 218)                 # demo_utils.EDGE_COLOR
 POSE_RECORD_INTS = 32                      # DAD3D_POSE_RECORD_INTS, include/dad3d.h
+MESH_WS_INTS = 5                           # DAD3D_MESH_WS_INTS
+# the vertex subset whose edges draw_mesh draws: head_edges.npy is over the face with ears, not flame_indices_head
+MESH_VERTICES = {"head_mesh": "flame_indices_face_w_ears", "face_mesh": "flame_indices_face"}
 _POINT_COLOR = np.array(POINT_COLOR, dtype=np.uint8)
+_EDGE_COLOR = np.array(EDGE_COLOR, dtype=np.uint8)
+
+
+def mesh_edges(faces: np.ndarray, vertices: np.ndarray) -> np.ndarray:
+    """[E,2] int32: the sorted unique (i < j) edges of the triangles ``faces`` with both ends in ``vertices``.  For the
+    FLAME faces and a subset of MESH_VERTICES this is, row for row, the reference's ``{subset}_edges.npy``."""
+    f = np.asarray(faces, dtype=np.int64)
+    e = np.unique(np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), axis=1), axis=0)
+    return np.ascontiguousarray(e[np.isin(e, np.asarray(vertices)).all(axis=1)], dtype=np.int32)
 
 
 def point_radius(height: int, width: int) -> int:
@@ -90,3 +105,21 @@ def draw_pose(frames: Tensor, pose: Tensor) -> None:
     with torch.cuda.device(frames.device):
         _lib.check(lib.dad3d_overlay_pose(pose.data_ptr(), int(pose.shape[0]), key.data_ptr(), frames.data_ptr(), F, H, W,
                                           _stream(frames.device)), "dad3d_overlay_pose")
+
+
+def draw_mesh(frames: Tensor, vertices: Tensor, rois: Tensor, edges: Tensor) -> None:
+    """In place on frames [F,H,W,3] uint8 (device): draw_mesh of every valid box's head onto its frame -- cv2.line(...,
+    1, LINE_AA) of every edge of ``edges`` [E,2] int32 in order, the blends of a pixel in box order.  ``vertices``
+    [R,N,2|3] fp32 (x, y truncated, as ``astype(int)``).  A box whose edges reach a point that is not finite or does not
+    fit int32 draws nothing."""
+    assert frames.dtype == torch.uint8 and frames.ndim == 4 and frames.is_contiguous()
+    assert vertices.dtype == torch.float32 and vertices.ndim == 3 and vertices.is_contiguous()
+    assert edges.dtype == torch.int32 and edges.ndim == 2 and edges.shape[1] == 2 and edges.is_contiguous()
+    F, H, W = (int(d) for d in frames.shape[:3])
+    R, N, C = (int(d) for d in vertices.shape)
+    ws = torch.empty(R, MESH_WS_INTS, dtype=torch.int32, device=frames.device)
+    lib = _lib.load()
+    with torch.cuda.device(frames.device):
+        _lib.check(lib.dad3d_overlay_mesh(vertices.data_ptr(), R, N, C, edges.data_ptr(), int(edges.shape[0]),
+                                          rois.data_ptr(), _EDGE_COLOR.ctypes.data, ws.data_ptr(), frames.data_ptr(), F, H,
+                                          W, _stream(frames.device)), "dad3d_overlay_mesh")

@@ -126,6 +126,7 @@ class FaceMeshPredictor:
         self._stride = config.get("stride", 2)
         self._static = None
         self._lm_index: Dict[str, Tensor] = {}
+        self._edges: Dict[str, Tensor] = {}
         self._graphs: Dict[Any, Any] = {}
         self._renderer: Optional[PnccRenderer] = None
         self._lit_renderer: Optional[LitRenderer] = None
@@ -274,6 +275,15 @@ class FaceMeshPredictor:
             self._lm_index[subset] = torch.from_numpy(self._static[key].astype(np.int64)).to(self.device)
         return self._lm_index[subset]
 
+    def _mesh_edges(self, kind: str) -> Tensor:
+        """draw_mesh's edge table of "head_mesh" / "face_mesh", derived from the packed faces and uploaded once."""
+        if kind not in self._edges:
+            if self._static is None:
+                self._static = load_flame_static()
+            e = overlay_ops.mesh_edges(self._static["faces"], self._static[overlay_ops.MESH_VERTICES[kind]])
+            self._edges[kind] = torch.from_numpy(e).to(self.device)
+        return self._edges[kind]
+
     @staticmethod
     def _render_keys(render, to_2d: bool) -> Tuple[str, ...]:
         """``render`` as a canonical tuple (the order of RENDER_KEYS), validated."""
@@ -420,6 +430,8 @@ class FaceMeshPredictor:
                     overlay_ops.draw_points(img, points, rois)
                 elif k == "pose":
                     overlay_ops.draw_pose(img, pose)
+                elif k in ("head_mesh", "face_mesh"):
+                    overlay_ops.draw_mesh(img, proj.contiguous(), rois, self._mesh_edges(k))
                 else:                                                 # the demo's "445" draws every file: the 565 set
                     subset = "191" if k == "191_landmarks" else "565"
                     overlay_ops.draw_points(img, proj.contiguous(), rois, self._landmark_index(subset))
@@ -466,8 +478,8 @@ class FaceMeshPredictor:
         nothing.  The reference's ``with_background=True`` overlay is, exactly,
         ``torch.where(out["frame_head_index"][..., None] >= 0, out["frame_pncc"], frames)``.
 
-        ``overlay`` (with ``boxes``): a subset of ("68_landmarks", "191_landmarks", "445_landmarks", "pose"), the demo's
-        ``type_of_output`` names.  Each adds "frame_<kind>" [F,H,W,3] uint8, a copy of the frames (never written) with that
+        ``overlay`` (with ``boxes``): a subset of ("68_landmarks", "191_landmarks", "445_landmarks", "pose", "head_mesh",
+        "face_mesh"), the demo's ``type_of_output`` names.  Each adds "frame_<kind>" [F,H,W,3] uint8, a copy of the frames (never written) with that
         overlay drawn by csrc/overlay.cu.  Frame f equals, byte for byte, a copy of frame f to which the reference's own
         processor from ``demo_utils.py`` is applied for every valid box on it, in box order, with that box's predictions:
         "68_landmarks" ``draw_landmarks({"points": points[r]}, copy)``; "191_landmarks" / "445_landmarks"
@@ -475,9 +487,13 @@ class FaceMeshPredictor:
         ``astype(int)`` and draws every file of the subset's directory -- so the demo's "445" draws the 565-point set
         (``keypoints_565``), and "191" the 191 set; "pose" ``draw_pose({"3dmm_params": params[r:r+1]}, copy[y:y+h, x:x+w])``
         into the crop view of ``crop_boxes[r]``: centre of the crop, arrow size h // 10, thickness int(h * 0.005), clipped at
-        the crop's border; later boxes, then later arrows (red, green, blue), win.  Where the reference has no defined
-        output, nothing is drawn: invalid boxes, points whose truncated coordinates are not finite or do not fit int32 (cv2
-        raises there), and the pose of a box whose crop is under 200 px high (thickness 0, which cv2.arrowedLine refuses;
+        the crop's border; later boxes, then later arrows (red, green, blue), win; "head_mesh" / "face_mesh"
+        ``draw_mesh({"projected_vertices": projected_vertices[r, :, :2]}, copy, subset)``, whose returned image is the
+        anti-aliased edges (cv2.line LINE_AA) of ``{subset}_edges.npy`` drawn in order, each pixel's blends in box, then edge
+        order -- the tables are derived from the packed faces (the edges over ``flame_indices_face_w_ears`` for "head", over
+        ``flame_indices_face`` for "face").  Where the reference has no defined output, nothing is drawn: invalid boxes,
+        points whose truncated coordinates are not finite or do not fit int32 (cv2 raises there; for the wireframes any such
+        end point of the subset's edges blanks that box's whole wireframe), and the pose of a box whose crop is under 200 px high (thickness 0, which cv2.arrowedLine refuses;
         its "rpy" is still written).  A whole image is the box [0, 0, W, H] with ``extend=0``.
 
         ``rpy=True`` adds "rpy" [B|R,3] float64, (roll, pitch, yaw) in degrees: ``calculate_rpy`` on each head's parameters

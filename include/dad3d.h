@@ -401,7 +401,7 @@ DAD3D_API int dad3d_render_lit(const float* vertices_d, int32_t nv, int32_t batc
                                dad3d_lighting lighting, const int32_t* image_of_head_d, int32_t n_images, int32_t h, int32_t w,
                                float* light_ws_d, uint8_t* image_d, unsigned long long* key_ws_d, dad3d_stream stream);
 
-/* ---- overlays: the demo's landmark and pose drawings, and head pose angles ----------------------------------------------
+/* ---- overlays: the demo's landmark, pose and wireframe drawings, and head pose angles ------------------------------
  * Draws what demo_utils.py's processors draw with cv2 (4.13.0; the rules are restated and pinned in tests/overlay_model.py),
  * byte for byte, into frames the caller has already copied, for R boxes at once, with every box-dependent value read on
  * the device from the dad3d_roi records (see "heads from boxes").  Invalid records draw nothing.
@@ -437,6 +437,17 @@ DAD3D_API int dad3d_overlay_points(const void* points_d, int32_t is_float, int32
                                    dad3d_stream stream);
 DAD3D_API int dad3d_overlay_pose(const int32_t* pose_d, int32_t R, int32_t* key_ws_d, uint8_t* frames_d, int32_t F,
                                  int32_t H, int32_t W, dad3d_stream stream);
+/*   dad3d_overlay_mesh  replaces draw_mesh (demo_utils.py:50-65): for every valid record r, cv2.line(frame, v[a], v[b],
+ *     color_h[3], 1, LINE_AA) for every edge (a, b) of edges_d [E,2] int32 in order, v being head r of vertices_d
+ *     [R,nv,ncomp] fp32 (ncomp 2 or 3; x, y truncated toward zero, as astype(int)), drawn into frames_d [F,H,W,3] frame
+ *     rois_d[r].frame.  The blends of one pixel come in (box, edge) order, as the reference's loop makes them.  A box draws
+ *     nothing when an end point of any edge is not finite or does not fit int32 (cv2 raises), or is outside [0, nv).
+ *     ws_d [R,DAD3D_MESH_WS_INTS] int32 is the caller's workspace: per box the frame it draws into (-1: none) and the pixel
+ *     box x0, y0, x1, y1 its stamps can touch.  Two kernels, no host synchronisation, 64-bit pixel offsets. */
+#define DAD3D_MESH_WS_INTS 5
+DAD3D_API int dad3d_overlay_mesh(const float* vertices_d, int32_t R, int32_t nv, int32_t ncomp, const int32_t* edges_d,
+                                 int32_t E, const dad3d_roi* rois_d, const uint8_t* color_h, int32_t* ws_d,
+                                 uint8_t* frames_d, int32_t F, int32_t H, int32_t W, dad3d_stream stream);
 
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
