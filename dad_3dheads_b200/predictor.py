@@ -12,6 +12,7 @@ also draws the PNCC, depth and triangle-index maps of every head (rasterizer.Pnc
 """
 from __future__ import annotations
 
+import dataclasses
 import logging
 import os
 from typing import Any, Dict, List, Optional, Tuple, Union
@@ -35,6 +36,9 @@ MAX_ROIS = 65535                                     # ROIs per call: dad3d_prep
 _FILENAME = "dad_3dheads.trcd"
 _MEAN = (0.485, 0.456, 0.406)
 _STD = (0.229, 0.224, 0.225)
+# the normalisation in pixel units, float32; the C entry points read them by value at call time (safe to capture)
+_MEAN_255 = np.array(_MEAN, dtype=np.float32) * 255.0
+_INV_STD_255 = np.reciprocal(np.array(_STD, dtype=np.float32) * 255.0, dtype=np.float32)
 RENDER_KEYS = ("pncc", "depth", "tri_index", "lit")
 FRAME_RENDER_KEYS = ("pncc", "depth", "tri_index", "head_index", "lit")    # predict_batch(boxes=, frame_render=) -> "frame_<key>"
 
@@ -81,14 +85,71 @@ def extend_sides(extend) -> Tuple[float, float, float, float]:
     return (float(extend),) * 4
 
 
+def _letterbox_size(h: int, w: int, img_size: int) -> Tuple[int, int]:
+    """LongestMaxSize's output size (h, w): the longer side scaled to ``img_size``, rounded as albumentations rounds."""
+    scale = img_size / float(max(h, w))
+    return (py3round(h * scale), py3round(w * scale)) if scale != 1.0 else (h, w)
+
+
+def _names(option: str, value, allowed: Tuple[str, ...], noun: str) -> Tuple[str, ...]:
+    """A name or a sequence of names -> a tuple in the order of ``allowed``; unknown names raise ValueError."""
+    if value is None:
+        return ()
+    given = {value} if isinstance(value, str) else set(value)
+    unknown = given - set(allowed)
+    if unknown:
+        raise ValueError(f"{option}: unknown {noun} {sorted(unknown)}; choose from {allowed}")
+    return tuple(k for k in allowed if k in given)
+
+
+@dataclasses.dataclass(frozen=True)
+class StepOptions:
+    """The options of one :meth:`FaceMeshPredictor.predict_batch` step, checked and in canonical form, so that equal
+    options give equal records: a record, with the input's shape and dtype, names one captured graph.
+
+    The fields take ``predict_batch``'s arguments.  After construction ``render``, ``frame_render`` and ``overlay`` are
+    tuples in the order of RENDER_KEYS, FRAME_RENDER_KEYS and OVERLAY_KINDS, ``rpy`` is a bool, ``rois`` is None (no
+    boxes) or the number of boxes per step, and ``extend`` is the four fractions of :func:`extend_sides` with boxes and
+    None without them (where it is ignored).  Unknown names and unsupported combinations raise ValueError."""
+    landmark_subset: Optional[str] = "445"
+    to_2d: bool = True
+    fast_decode: bool = True
+    render: Tuple[str, ...] = ()
+    frame_render: Tuple[str, ...] = ()
+    overlay: Tuple[str, ...] = ()
+    rpy: bool = False
+    rois: Optional[int] = None
+    extend: Any = 0.0
+
+    def __post_init__(self):
+        render = _names("render", self.render, RENDER_KEYS, "maps")
+        frame_render = _names("frame_render", self.frame_render, FRAME_RENDER_KEYS, "maps")
+        overlay = _names("overlay", self.overlay, OVERLAY_KINDS, "kinds")
+        boxes = self.rois is not None
+        if render and self.to_2d:
+            raise ValueError("render needs to_2d=False: the renderer takes the projected vertices with their depth")
+        if frame_render and not boxes:
+            raise ValueError("frame_render needs boxes: it draws the heads of each box into its frame")
+        if frame_render and self.to_2d:
+            raise ValueError("frame_render needs to_2d=False: the renderer takes the projected vertices with their depth")
+        if overlay and not boxes:
+            raise ValueError("overlay needs boxes: it draws into copies of the frames, which the no-box path does not have")
+        if render and boxes:
+            raise ValueError("render is not supported together with boxes")
+        canonical = dict(to_2d=bool(self.to_2d), fast_decode=bool(self.fast_decode), render=render,
+                         frame_render=frame_render, overlay=overlay, rpy=bool(self.rpy),
+                         rois=int(self.rois) if boxes else None, extend=extend_sides(self.extend) if boxes else None)
+        for name, value in canonical.items():
+            object.__setattr__(self, name, value)
+
+
 def letterbox_normalise(x: np.ndarray, img_size: int) -> np.ndarray:
     """predictor.py:195-203 (albumentations 1.0.0 LongestMaxSize -> PadIfNeeded(constant 0, centred) -> Normalize),
     restated with cv2/numpy: HxWx3 uint8 RGB -> img_size x img_size x 3 float32."""
     import cv2
     h, w = x.shape[:2]
-    scale = img_size / float(max(w, h))
-    if scale != 1.0:
-        nh, nw = py3round(h * scale), py3round(w * scale)
+    nh, nw = _letterbox_size(h, w, img_size)
+    if (nh, nw) != (h, w):
         x = cv2.resize(x, dsize=(nw, nh), interpolation=cv2.INTER_LINEAR)
     h, w = x.shape[:2]
     top = int((img_size - h) / 2.0) if h < img_size else 0
@@ -97,11 +158,9 @@ def letterbox_normalise(x: np.ndarray, img_size: int) -> np.ndarray:
     right = (img_size - w - left) if w < img_size else 0
     if top or bottom or left or right:
         x = cv2.copyMakeBorder(x, top, bottom, left, right, cv2.BORDER_CONSTANT, value=0)
-    mean = np.array(_MEAN, dtype=np.float32) * 255.0
-    denom = np.reciprocal(np.array(_STD, dtype=np.float32) * 255.0, dtype=np.float32)
     out = x.astype(np.float32)
-    out -= mean
-    out *= denom
+    out -= _MEAN_255
+    out *= _INV_STD_255
     return out
 
 
@@ -127,7 +186,7 @@ class FaceMeshPredictor:
         self._static = None
         self._lm_index: Dict[str, Tensor] = {}
         self._edges: Dict[str, Tensor] = {}
-        self._graphs: Dict[Any, Any] = {}
+        self._graphs: Dict[Any, CapturedStep] = {}
         self._renderer: Optional[PnccRenderer] = None
         self._lit_renderer: Optional[LitRenderer] = None
 
@@ -234,20 +293,18 @@ class FaceMeshPredictor:
         pixels cross the PCIe bus."""
         lib = _lib.load()
         S = self._img_size
-        mean = (np.array(_MEAN, dtype=np.float32) * 255.0).astype(np.float32)
-        inv = np.reciprocal(np.array(_STD, dtype=np.float32) * 255.0, dtype=np.float32)
+        mean, inv = _MEAN_255.ctypes.data, _INV_STD_255.ctypes.data
         stream = torch.cuda.current_stream(self.device).cuda_stream
         if isinstance(images, Tensor) and images.ndim == 4:
             # one [B,H,W,3] uint8 tensor (host, ideally pinned, or device): one copy, one launch
             assert images.dtype == torch.uint8 and images.shape[3] == 3
             B, h, w = int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
-            scale = S / float(max(h, w))
-            nh, nw = (py3round(h * scale), py3round(w * scale)) if scale != 1.0 else (h, w)
+            nh, nw = _letterbox_size(h, w, S)
             out = torch.empty(B, 3, S, S, dtype=torch.float32, device=self.device)
             with torch.cuda.device(self.device):
                 d = images.contiguous().to(self.device, non_blocking=True)
-                _lib.check(lib.dad3d_preprocess_batch(d.data_ptr(), B, h, w, nh, nw, S, mean.ctypes.data, inv.ctypes.data,
-                                                      out.data_ptr(), stream), "dad3d_preprocess_batch")
+                _lib.check(lib.dad3d_preprocess_batch(d.data_ptr(), B, h, w, nh, nw, S, mean, inv, out.data_ptr(), stream),
+                           "dad3d_preprocess_batch")
                 d.record_stream(torch.cuda.current_stream(self.device))
             return out
         out = torch.empty(len(images), 3, S, S, dtype=torch.float32, device=self.device)
@@ -257,12 +314,11 @@ class FaceMeshPredictor:
                 t = torch.as_tensor(im)
                 assert t.dtype == torch.uint8 and t.ndim == 3 and t.shape[2] == 3
                 h, w = int(t.shape[0]), int(t.shape[1])
-                scale = S / float(max(h, w))
-                nh, nw = (py3round(h * scale), py3round(w * scale)) if scale != 1.0 else (h, w)
+                nh, nw = _letterbox_size(h, w, S)
                 d = t.contiguous().to(self.device, non_blocking=True)
                 keep.append(d)
-                _lib.check(lib.dad3d_preprocess(d.data_ptr(), h, w, nh, nw, S, mean.ctypes.data, inv.ctypes.data,
-                                                out[i].data_ptr(), stream), "dad3d_preprocess")
+                _lib.check(lib.dad3d_preprocess(d.data_ptr(), h, w, nh, nw, S, mean, inv, out[i].data_ptr(), stream),
+                           "dad3d_preprocess")
         return out
 
     # ------------------------------------------------------------------ batched device-resident API (new)
@@ -283,53 +339,6 @@ class FaceMeshPredictor:
             e = overlay_ops.mesh_edges(self._static["faces"], self._static[overlay_ops.MESH_VERTICES[kind]])
             self._edges[kind] = torch.from_numpy(e).to(self.device)
         return self._edges[kind]
-
-    @staticmethod
-    def _render_keys(render, to_2d: bool) -> Tuple[str, ...]:
-        """``render`` as a canonical tuple (the order of RENDER_KEYS), validated."""
-        if render is None:
-            return ()
-        if isinstance(render, str):
-            render = (render,)
-        unknown = set(render) - set(RENDER_KEYS)
-        if unknown:
-            raise ValueError(f"render: unknown maps {sorted(unknown)}; choose from {RENDER_KEYS}")
-        keys = tuple(k for k in RENDER_KEYS if k in render)
-        if keys and to_2d:
-            raise ValueError("render needs to_2d=False: the renderer takes the projected vertices with their depth")
-        return keys
-
-    @staticmethod
-    def _frame_render_keys(frame_render, to_2d: bool, boxes) -> Tuple[str, ...]:
-        """``frame_render`` as a canonical tuple (the order of FRAME_RENDER_KEYS), validated against ``to_2d`` and ``boxes``."""
-        if frame_render is None:
-            return ()
-        if isinstance(frame_render, str):
-            frame_render = (frame_render,)
-        unknown = set(frame_render) - set(FRAME_RENDER_KEYS)
-        if unknown:
-            raise ValueError(f"frame_render: unknown maps {sorted(unknown)}; choose from {FRAME_RENDER_KEYS}")
-        keys = tuple(k for k in FRAME_RENDER_KEYS if k in frame_render)
-        if keys and boxes is None:
-            raise ValueError("frame_render needs boxes: it draws the heads of each box into its frame")
-        if keys and to_2d:
-            raise ValueError("frame_render needs to_2d=False: the renderer takes the projected vertices with their depth")
-        return keys
-
-    @staticmethod
-    def _overlay_keys(overlay, boxes) -> Tuple[str, ...]:
-        """``overlay`` as a canonical tuple (the order of OVERLAY_KINDS), validated against ``boxes``."""
-        if overlay is None:
-            return ()
-        if isinstance(overlay, str):
-            overlay = (overlay,)
-        unknown = set(overlay) - set(OVERLAY_KINDS)
-        if unknown:
-            raise ValueError(f"overlay: unknown kinds {sorted(unknown)}; choose from {OVERLAY_KINDS}")
-        keys = tuple(k for k in OVERLAY_KINDS if k in overlay)
-        if keys and boxes is None:
-            raise ValueError("overlay needs boxes: it draws into copies of the frames, which the no-box path does not have")
-        return keys
 
     def _rotation_index(self) -> int:
         """Where FlameParams.from_3dmm (model/flame.py:41-101) reads the six rotation parameters."""
@@ -371,11 +380,10 @@ class FaceMeshPredictor:
             raise ValueError("boxes need the released 3DMM layout (one scale, three translation parameters)")
         return boxes, frame_index
 
-    def _predict_rois(self, frames, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
-                      frame_render=(), overlay=(), rpy=False) -> Dict[str, Tensor]:
-        """predict_batch with boxes: crop geometry, pre-processing and read-back in csrc/roi.cu, no host synchronisation."""
-        boxes, frame_index = self._check_rois(frames, boxes, frame_index)
-        ext = np.array(extend_sides(extend), dtype=np.float64)
+    def _roi_input(self, frames: Tensor, boxes: Tensor, frame_index: Optional[Tensor], extend) -> Tuple[Tensor, ...]:
+        """The input stage of predict_batch with boxes: crop geometry, pre-processing, encoder and read-back to frame
+        pixels (csrc/roi.cu), no host synchronisation -> (frames on the device, [R,72] dad3d_roi records, params, points)."""
+        ext = np.array(extend, dtype=np.float64)
         frames = frames.to(self.device, non_blocking=True).contiguous()
         boxes = boxes.to(self.device, torch.int32, non_blocking=True).contiguous()
         if frame_index is not None:
@@ -385,16 +393,14 @@ class FaceMeshPredictor:
         S = self._img_size
         F, H, W = (int(d) for d in frames.shape[:3])
         R = int(boxes.shape[0])
-        mean = (np.array(_MEAN, dtype=np.float32) * 255.0).astype(np.float32)
-        inv = np.reciprocal(np.array(_STD, dtype=np.float32) * 255.0, dtype=np.float32)
         rois = torch.empty(R, ROI_RECORD_BYTES, dtype=torch.uint8, device=self.device)
         x = torch.empty(R, 3, S, S, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             stream = torch.cuda.current_stream(self.device).cuda_stream
             _lib.check(lib.dad3d_roi_setup(boxes.data_ptr(), frame_index.data_ptr() if frame_index is not None else None, R,
                                            F, H, W, S, ext.ctypes.data, rois.data_ptr(), stream), "dad3d_roi_setup")
-            _lib.check(lib.dad3d_preprocess_rois(frames.data_ptr(), H, W, rois.data_ptr(), R, S, mean.ctypes.data,
-                                                 inv.ctypes.data, x.data_ptr(), stream), "dad3d_preprocess_rois")
+            _lib.check(lib.dad3d_preprocess_rois(frames.data_ptr(), H, W, rois.data_ptr(), R, S, _MEAN_255.ctypes.data,
+                                                 _INV_STD_255.ctypes.data, x.data_ptr(), stream), "dad3d_preprocess_rois")
             raw, lms, _ = self.model.forward_raw(x, want_heatmap=False)
             params = torch.empty_like(raw)
             points = torch.empty(R, lms.shape[1], 2, dtype=torch.int64, device=self.device)
@@ -402,14 +408,38 @@ class FaceMeshPredictor:
                                                lms.shape[1], self.find_3dmm_idx("scale", c),
                                                self.find_3dmm_idx("translation", c), S, params.data_ptr(),
                                                points.data_ptr(), stream), "dad3d_readjust_rois")
-        v3, proj = self.head_mesh.decode(params, to_2d=to_2d, hilo=not fast_decode)
-        fields = rois.view(torch.int32)                       # x, y, w, h, frame, valid, ... (dad3d_roi)
-        out = {"3dmm_params": params, "points": points, "3d_vertices": v3, "projected_vertices": proj,
-               "crop_boxes": fields[:, :4].contiguous(), "valid": fields[:, 5] != 0}
-        if landmark_subset is not None:
+        return frames, rois, params, points
+
+    def _step(self, images, opts: StepOptions, boxes: Optional[Tensor] = None,
+              frame_index: Optional[Tensor] = None) -> Dict[str, Tensor]:
+        """One predict_batch step on checked arguments (``_check_rois``), without host synchronisation, so a capture runs
+        it as well: the input stage of the path, the decode, then the output stage both paths share."""
+        rois = None
+        if opts.rois is None:
+            if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
+                x = self.preprocess_batch(images)
+            else:
+                x = images.to(self.device, torch.float32, non_blocking=True)
+            params, lms, _ = self.model.forward_raw(x, want_heatmap=False)
+            points = lms * float(self._img_size)
+        else:
+            frames, rois, params, points = self._roi_input(images, boxes, frame_index, opts.extend)
+        v3, proj = self.head_mesh.decode(params, to_2d=opts.to_2d, hilo=not opts.fast_decode)
+        out = {"3dmm_params": params, "points": points, "3d_vertices": v3, "projected_vertices": proj}
+        if rois is not None:
+            fields = rois.view(torch.int32)                       # x, y, w, h, frame, valid, ... (dad3d_roi)
+            out.update({"crop_boxes": fields[:, :4].contiguous(), "valid": fields[:, 5] != 0})
+        if opts.landmark_subset is not None:
             dec = self.head_mesh.flame.decoder(self.device)
-            out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
+            out[f"landmarks_{opts.landmark_subset}"] = dec.gather(proj, self._landmark_index(opts.landmark_subset))
+        render, frame_render, overlay = opts.render, opts.frame_render, opts.overlay
+        if set(render) - {"lit"}:
+            out.update(self._pncc_renderer()(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
+                                             tri_index="tri_index" in render))
+        if "lit" in render:
+            out.update(self._lit()(proj, self._img_size))
         if frame_render:
+            F, H, W = (int(d) for d in frames.shape[:3])
             frame_of_head = torch.where(out["valid"], fields[:, 4], -1)            # invalid boxes draw nothing
             if set(frame_render) - {"lit"}:
                 maps = self._pncc_renderer().render_frames(proj, frame_of_head, F, (H, W), pncc="pncc" in frame_render,
@@ -419,23 +449,22 @@ class FaceMeshPredictor:
                 out.update({f"frame_{k}": t for k, t in maps.items()})
             if "lit" in frame_render:
                 out["frame_lit"] = self._lit().render_frames(proj, frame_of_head, F, (H, W), frames=frames)["lit"]
-        if rpy or "pose" in overlay:
+        if opts.rpy or "pose" in overlay:
             angles, pose = overlay_ops.pose_geometry(params, self._rotation_index(), rois if "pose" in overlay else None)
-            if rpy:
+            if opts.rpy:
                 out["rpy"] = angles
-        if overlay:
-            copies = {k: frames.clone() for k in overlay}            # one device copy per kind, before any drawing
-            for k, img in copies.items():
-                if k == "68_landmarks":
-                    overlay_ops.draw_points(img, points, rois)
-                elif k == "pose":
-                    overlay_ops.draw_pose(img, pose)
-                elif k in ("head_mesh", "face_mesh"):
-                    overlay_ops.draw_mesh(img, proj.contiguous(), rois, self._mesh_edges(k))
-                else:                                                 # the demo's "445" draws every file: the 565 set
-                    subset = "191" if k == "191_landmarks" else "565"
-                    overlay_ops.draw_points(img, proj.contiguous(), rois, self._landmark_index(subset))
-                out[f"frame_{k}"] = img
+        copies = {k: frames.clone() for k in overlay}                # one device copy per kind, before any drawing
+        for k, img in copies.items():
+            if k == "68_landmarks":
+                overlay_ops.draw_points(img, points, rois)
+            elif k == "pose":
+                overlay_ops.draw_pose(img, pose)
+            elif k in ("head_mesh", "face_mesh"):
+                overlay_ops.draw_mesh(img, proj.contiguous(), rois, self._mesh_edges(k))
+            else:                                                     # the demo's "445" draws every file: the 565 set
+                subset = "191" if k == "191_landmarks" else "565"
+                overlay_ops.draw_points(img, proj.contiguous(), rois, self._landmark_index(subset))
+            out[f"frame_{k}"] = img
         return out
 
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
@@ -499,71 +528,16 @@ class FaceMeshPredictor:
         ``rpy=True`` adds "rpy" [B|R,3] float64, (roll, pitch, yaw) in degrees: ``calculate_rpy`` on each head's parameters
         (the reference computes head 0 only), to ~1e-12 degrees away from gimbal lock (scipy's SVD polar factor of the
         fp32 rotation is taken by Newton steps on the device).  With boxes, the rotation is that of the crop: the read-back does not change it."""
-        render = self._render_keys(render, to_2d)
-        frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
-        overlay = self._overlay_keys(overlay, boxes)
         if boxes is not None:
-            if render:
-                raise ValueError("render is not supported together with boxes")
-            return self._predict_rois(images, boxes, frame_index, extend, landmark_subset, to_2d, fast_decode,
-                                      frame_render, overlay, bool(rpy))
-        if isinstance(images, (list, tuple)) or (isinstance(images, Tensor) and images.dtype == torch.uint8):
-            x = self.preprocess_batch(images)
-        else:
-            x = images.to(self.device, torch.float32, non_blocking=True)
-        params, lms, _ = self.model.forward_raw(x, want_heatmap=False)
-        v3, proj = self.head_mesh.decode(params, to_2d=to_2d, hilo=not fast_decode)
-        out = {"3dmm_params": params, "points": lms * float(self._img_size), "3d_vertices": v3,
-               "projected_vertices": proj}
-        if landmark_subset is not None:
-            dec = self.head_mesh.flame.decoder(self.device)
-            out[f"landmarks_{landmark_subset}"] = dec.gather(proj, self._landmark_index(landmark_subset))
-        if set(render) - {"lit"}:
-            out.update(self._pncc_renderer()(proj, self._img_size, pncc="pncc" in render, depth="depth" in render,
-                                      tri_index="tri_index" in render))
-        if "lit" in render:
-            out.update(self._lit()(proj, self._img_size))
-        if rpy:
-            out["rpy"] = overlay_ops.pose_geometry(params, self._rotation_index())[0]
-        return out
+            boxes, frame_index = self._check_rois(images, boxes, frame_index)
+        opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy,
+                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend)
+        return self._step(images, opts, boxes, frame_index)
 
     def _ws_generation(self):
         """Changes whenever the encoder or decoder scratch buffer is reallocated (captured graphs bake in its address)."""
         dec = self.head_mesh.flame.decoder(self.device)
         return (self.model.ws_generation, dec.ws_generation)
-
-    def _capture(self, static_in: Tensor, landmark_subset, to_2d, fast_decode, render=None, rois=None, frame_render=(),
-                 overlay=(), rpy=False):
-        """Warm up (plans, workspaces, tensor maps, index tables) and capture predict_batch(static_in) into a CUDA graph.
-        ``rois`` = (static boxes [R,4] int32, static frame index [R] int32, extend): the graph reads the boxes from those
-        buffers on every replay."""
-        kw = dict(boxes=rois[0], frame_index=rois[1], extend=rois[2], frame_render=frame_render,
-                  overlay=overlay) if rois is not None else {}
-        kw["rpy"] = rpy
-        side = torch.cuda.Stream(self.device)
-        side.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render, **kw)
-        torch.cuda.current_stream(self.device).wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            out = self.predict_batch(static_in, landmark_subset, to_2d, fast_decode, render, **kw)
-        return graph, out, self._ws_generation()
-
-    def _roi_buffers(self, R: int, extend):
-        """Static boxes / frame index buffers of a captured step with R boxes (zero boxes: every ROI invalid until filled)."""
-        return (torch.zeros(R, 4, dtype=torch.int32, device=self.device),
-                torch.zeros(R, dtype=torch.int32, device=self.device), extend_sides(extend))
-
-    @staticmethod
-    def _fill_rois(rois, boxes: Tensor, frame_index: Optional[Tensor]) -> None:
-        rois[0].copy_(boxes, non_blocking=True)
-        if frame_index is None:
-            rois[1].zero_()
-        else:
-            rois[1].copy_(frame_index, non_blocking=True)
 
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                               fast_decode: bool = True, render=None, boxes=None, frame_index=None,
@@ -580,42 +554,79 @@ class FaceMeshPredictor:
         With ``boxes`` (see :meth:`predict_batch`) the boxes and frame indices are copied into static buffers as well: one
         graph serves every box set of the same frame shape, box count, ``extend``, ``frame_render`` and ``overlay``."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
-        render = self._render_keys(render, to_2d)
-        frame_render = self._frame_render_keys(frame_render, to_2d, boxes)
-        overlay = self._overlay_keys(overlay, boxes)
-        rpy = bool(rpy)
-        key = (tuple(images.shape), images.dtype, landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy)
         if boxes is not None:
-            if render:
-                raise ValueError("render is not supported together with boxes")
             boxes, frame_index = self._check_rois(images, boxes, frame_index)
-            key += (int(boxes.shape[0]), extend_sides(extend))
-        ent = self._graphs.get(key)
-        if ent is not None and ent[3] != self._ws_generation():
-            ent = None                                        # scratch moved since the capture: never replay it
-            self._graphs.pop(key)
-        if ent is None:
-            static_in = torch.empty(images.shape, dtype=images.dtype, device=self.device)
-            static_in.copy_(images, non_blocking=True)
-            rois = self._roi_buffers(int(boxes.shape[0]), extend) if boxes is not None else None
-            if rois is not None:
-                self._fill_rois(rois, boxes, frame_index)
-            graph, out, gen = self._capture(static_in, landmark_subset, to_2d, fast_decode, render, rois, frame_render,
-                                            overlay, rpy)
-            ent = (graph, static_in, out, gen, rois)
-            self._graphs[key] = ent
-        graph, static_in, out, _, rois = ent
-        static_in.copy_(images, non_blocking=True)
-        if rois is not None:
-            self._fill_rois(rois, boxes, frame_index)
-        graph.replay()
-        return out
+        opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy,
+                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend)
+        key = (opts, tuple(images.shape), images.dtype)
+        step = self._graphs.get(key)
+        if step is None:
+            step = self._graphs[key] = CapturedStep(self, opts, images.shape, images.dtype)
+        step.load(images, boxes, frame_index)
+        if step.stale():
+            step.capture()
+        step.graph.replay()
+        return step.out
 
     def open_stream(self, shape, dtype=torch.uint8, **kw) -> "BatchStream":
         """A double-buffered pipeline over :meth:`predict_batch` for a fixed batch signature -- see :class:`BatchStream`.
         ``rois=R`` (with optional ``extend``, ``frame_render`` and ``overlay``): ``shape`` is that of the frames, and every submit
         brings R boxes.  ``rpy`` is passed to ``predict_batch``."""
         return BatchStream(self, shape, dtype, **kw)
+
+
+class CapturedStep:
+    """One predict_batch step captured into a CUDA graph: its static input, box and frame-index buffers, the graph, its
+    outputs and the scratch generation it was captured at.
+
+    The graph holds raw pointers into the encoder / decoder scratch buffers.  Those buffers only ever grow; once one has
+    been reallocated (a larger batch, eager or graphed), the graph is :meth:`stale` and must be captured again before it is
+    replayed, so a stale pointer is never dereferenced."""
+
+    def __init__(self, predictor: FaceMeshPredictor, opts: StepOptions, shape, dtype):
+        self.pred = predictor
+        self.opts = opts
+        dev = predictor.device
+        self.input = torch.zeros(tuple(shape), dtype=dtype, device=dev)
+        self.boxes = self.frame_index = None
+        if opts.rois is not None:                            # zero boxes: every ROI invalid until loaded
+            self.boxes = torch.zeros(opts.rois, 4, dtype=torch.int32, device=dev)
+            self.frame_index = torch.zeros(opts.rois, dtype=torch.int32, device=dev)
+            predictor._check_rois(self.input, self.boxes, self.frame_index)     # the frame shape and the 3DMM layout
+        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.out: Dict[str, Tensor] = {}
+        self.generation = None
+
+    def load(self, images: Tensor, boxes: Optional[Tensor] = None, frame_index: Optional[Tensor] = None) -> None:
+        """Copies a step's inputs into the static buffers, on the current stream (frame_index None: every box on frame 0)."""
+        self.input.copy_(images, non_blocking=True)
+        if boxes is not None:
+            self.boxes.copy_(boxes, non_blocking=True)
+            if frame_index is None:
+                self.frame_index.zero_()
+            else:
+                self.frame_index.copy_(frame_index, non_blocking=True)
+
+    def stale(self) -> bool:
+        """True before the first capture, and once the scratch buffers of the capture have been reallocated."""
+        return self.generation != self.pred._ws_generation()
+
+    def capture(self) -> None:
+        """Warms up (plans, workspaces, tensor maps, index tables) on a side stream, then captures the step on the static
+        buffers, which the graph reads on every replay."""
+        pred, dev = self.pred, self.pred.device
+        self.graph = self.generation = None                  # the stale graph's memory goes back before the new capture
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                pred._step(self.input, self.opts, self.boxes, self.frame_index)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            self.out = pred._step(self.input, self.opts, self.boxes, self.frame_index)
+        self.graph, self.generation = graph, pred._ws_generation()
 
 
 class BatchStream:
@@ -638,6 +649,8 @@ class BatchStream:
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
                  group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None, rois=None,
                  extend=0.0, frame_render=None, overlay=None, rpy: bool = False):
+        self.opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy, rois=rois,
+                                extend=extend)
         self.pred = predictor
         dev = predictor.device
         self.device = dev
@@ -651,21 +664,13 @@ class BatchStream:
         self.copy_in = torch.cuda.Stream(dev)
         self.copy_out = torch.cuda.Stream(dev)
         self.comm = torch.cuda.Stream(dev) if group is not None else None
-        self._args = (landmark_subset, to_2d, fast_decode, predictor._render_keys(render, to_2d))
-        if rois is not None and self._args[3]:
-            raise ValueError("render is not supported together with boxes")
-        self._frame_render = predictor._frame_render_keys(frame_render, to_2d, rois)
-        self._overlay = predictor._overlay_keys(overlay, rois)
-        self._rpy = bool(rpy)
-        self.rois = rois
         self.slots = []
         with torch.cuda.device(dev):
             for _ in range(self.depth):
-                static_in = torch.zeros(tuple(shape), dtype=dtype, device=dev)
-                roi_bufs = predictor._roi_buffers(int(rois), extend) if rois is not None else None
-                graph, out, gen = predictor._capture(static_in, *self._args, roi_bufs, self._frame_render, self._overlay,
-                                                     self._rpy)
-                slot = {"in": static_in, "rois": roi_bufs, "graph": graph, "out": out, "gen": gen, "busy": False,
+                step = CapturedStep(predictor, self.opts, shape, dtype)
+                step.capture()
+                out = step.out
+                slot = {"step": step, "out": out, "busy": False,
                         "h2d": torch.cuda.Event(), "done": torch.cuda.Event(), "comm_done": torch.cuda.Event(),
                         "d2h": torch.cuda.Event(), "gathered": {}, "host": {}}
                 if host_results:
@@ -687,29 +692,29 @@ class BatchStream:
     def submit(self, images: Tensor, boxes=None, frame_index=None) -> None:
         if self._inflight == self.depth:
             raise RuntimeError("BatchStream: all slots in flight -- collect() before submitting more")
-        if (boxes is None) != (self.rois is None):
+        rois = self.opts.rois
+        if (boxes is None) != (rois is None):
             raise ValueError("boxes are required exactly when the stream was opened with rois=")
         if boxes is not None:
             boxes, frame_index = self.pred._check_rois(images, boxes, frame_index)
-            if int(boxes.shape[0]) != self.rois:
-                raise ValueError(f"boxes: this stream takes {self.rois} per batch, got {int(boxes.shape[0])}")
+            if int(boxes.shape[0]) != rois:
+                raise ValueError(f"boxes: this stream takes {rois} per batch, got {int(boxes.shape[0])}")
         s = self.slots[self._head]
-        if s["gen"] != self.pred._ws_generation():           # scratch reallocated by another caller: re-capture this slot
+        step = s["step"]
+        if step.stale():                                      # scratch reallocated by another caller: re-capture this slot
             torch.cuda.synchronize(self.device)
-            s["graph"], s["out"], s["gen"] = self.pred._capture(s["in"], *self._args, s["rois"], self._frame_render,
-                                                                self._overlay, self._rpy)
+            step.capture()
+            s["out"] = step.out                              # the slot's outputs are the new graph's
         with torch.cuda.stream(self.copy_in):
             self.copy_in.wait_event(s["done"])               # the previous replay of this slot has consumed its input
-            s["in"].copy_(images, non_blocking=True)
-            if boxes is not None:
-                self.pred._fill_rois(s["rois"], boxes, frame_index)
+            step.load(images, boxes, frame_index)
             s["h2d"].record(self.copy_in)
         with torch.cuda.stream(self.compute):
             self.compute.wait_event(s["h2d"])
             self.compute.wait_event(s["d2h"])                # its previous results have left the device buffers
             if self.comm is not None:
                 self.compute.wait_event(s["comm_done"])
-            s["graph"].replay()
+            step.graph.replay()
             s["done"].record(self.compute)
         last = s["done"]
         if self.comm is not None:

@@ -101,6 +101,32 @@ def _check_triangles(triangles: torch.Tensor, nv: int) -> None:
     triangles._dad3d_checked = tag
 
 
+def _image_map(image_of_head: Optional[torch.Tensor], num_images: Optional[int], B: int, ntri: int, dev):
+    """Checks a head -> image map of B heads of ``ntri`` triangles -> (the number of output images, the map made
+    contiguous); without a map, B images and None."""
+    if (image_of_head is not None) != (num_images is not None):
+        raise ValueError("image_of_head and num_images go together")
+    if image_of_head is None:
+        return B, None
+    if image_of_head.shape != (B,) or image_of_head.dtype != torch.int32 or image_of_head.device != dev:
+        raise ValueError(f"image_of_head must be a [{B}] int32 tensor on the vertices' device")
+    n_out = int(num_images)
+    if n_out < 0:
+        raise ValueError(f"num_images must be >= 0, got {n_out}")
+    if B * ntri > 2 ** 32 - 2:
+        raise ValueError(f"{B} heads x {ntri} triangles exceed 2^32 - 2 (head, triangle) pairs")
+    return n_out, image_of_head.contiguous()
+
+
+def _output_image(image: Optional[torch.Tensor], n: int, height: int, width: int, c: int, dev) -> torch.Tensor:
+    """The image the heads are drawn over: zeros, or a copy of ``image`` ([n,height,width,c] uint8) on ``dev``."""
+    if image is None:
+        return torch.zeros(n, height, width, c, dtype=torch.uint8, device=dev)
+    if tuple(image.shape) != (n, height, width, c) or image.dtype != torch.uint8:
+        raise ValueError(f"image must be [{n},{height},{width},{c}] uint8")
+    return image.to(dev, copy=True).contiguous()
+
+
 def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Optional[torch.Tensor] = None, *, height: int,
                     width: int, image: Optional[torch.Tensor] = None, depth: bool = True, tri_index: bool = True,
                     reverse: bool = False, negate_z: bool = False, image_of_head: Optional[torch.Tensor] = None,
@@ -130,20 +156,9 @@ def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Opt
     if nv == 0 or height <= 0 or width <= 0 or height * width >= 1 << 31:
         raise ValueError(f"bad shape: nv={nv}, height={height}, width={width}")
     mapped = image_of_head is not None
-    if mapped != (num_images is not None):
-        raise ValueError("image_of_head and num_images go together")
-    n_out = B
-    if mapped:
-        if image_of_head.shape != (B,) or image_of_head.dtype != torch.int32 or image_of_head.device != dev:
-            raise ValueError(f"image_of_head must be a [{B}] int32 tensor on the vertices' device")
-        if reverse:
-            raise ValueError("reverse is not available with image_of_head")
-        n_out = int(num_images)
-        if n_out < 0:
-            raise ValueError(f"num_images must be >= 0, got {n_out}")
-        if B * int(triangles.shape[0]) > 2 ** 32 - 2:
-            raise ValueError(f"{B} heads x {int(triangles.shape[0])} triangles exceed 2^32 - 2 (head, triangle) pairs")
-        image_of_head = image_of_head.contiguous()
+    n_out, image_of_head = _image_map(image_of_head, num_images, B, int(triangles.shape[0]), dev)
+    if mapped and reverse:
+        raise ValueError("reverse is not available with image_of_head")
     vertices = vertices.contiguous()
     triangles = triangles.contiguous()
     _check_triangles(triangles, nv)
@@ -154,12 +169,7 @@ def rasterize_batch(vertices: torch.Tensor, triangles: torch.Tensor, colors: Opt
             raise ValueError("colors must be an [nv,C] float32 tensor on the vertices' device")
         colors = colors.contiguous()
         c = int(colors.shape[1])
-        if image is None:
-            out["image"] = torch.zeros(n_out, height, width, c, dtype=torch.uint8, device=dev)
-        else:
-            if tuple(image.shape) != (n_out, height, width, c) or image.dtype != torch.uint8:
-                raise ValueError(f"image must be [{n_out},{height},{width},{c}] uint8")
-            out["image"] = image.to(dev, copy=True).contiguous()
+        out["image"] = _output_image(image, n_out, height, width, c, dev)
     elif image is not None:
         raise ValueError("image needs colors")
     if depth:
@@ -222,15 +232,20 @@ class PnccRenderer:
         self.colors = torch.from_numpy(st["ncc_colors"]).to(self.device)
         _check_triangles(self.faces, int(self.colors.shape[0]))
 
-    def __call__(self, projected_vertices_3d: torch.Tensor, size: int, *, pncc: bool = True, depth: bool = True,
-                 tri_index: bool = True) -> Dict[str, torch.Tensor]:
+    def _render(self, projected_vertices_3d: torch.Tensor, size, pncc: bool, **kw) -> Dict[str, torch.Tensor]:
+        """rasterize_batch of [B,nv,3] vertices at ``size`` = (H, W), z negated, with "image" named "pncc"."""
         if projected_vertices_3d.ndim != 3 or projected_vertices_3d.shape[1:] != (self.colors.shape[0], 3):
             raise ValueError(f"expected [B,{self.colors.shape[0]},3] vertices, got {tuple(projected_vertices_3d.shape)}")
-        out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=size, width=size,
-                              depth=depth, tri_index=tri_index, negate_z=True)
+        height, width = (int(v) for v in size)
+        out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=height, width=width,
+                              negate_z=True, **kw)
         if pncc:
             out["pncc"] = out.pop("image")
         return out
+
+    def __call__(self, projected_vertices_3d: torch.Tensor, size: int, *, pncc: bool = True, depth: bool = True,
+                 tri_index: bool = True) -> Dict[str, torch.Tensor]:
+        return self._render(projected_vertices_3d, (size, size), pncc, depth=depth, tri_index=tri_index)
 
     def render_frames(self, projected_vertices_3d: torch.Tensor, frame_of_head: torch.Tensor, num_frames: int, size, *,
                       pncc: bool = True, depth: bool = True, tri_index: bool = True,
@@ -246,15 +261,8 @@ class PnccRenderer:
         image and depth buffer: the nearest surface wins across heads, and an exact depth tie goes to the lower head.  The
         reference's ``with_background=True`` overlay is ``torch.where(head_index[..., None] >= 0, pncc, frames)``, exactly,
         since alpha = 1 overwrites every covered pixel."""
-        if projected_vertices_3d.ndim != 3 or projected_vertices_3d.shape[1:] != (self.colors.shape[0], 3):
-            raise ValueError(f"expected [B,{self.colors.shape[0]},3] vertices, got {tuple(projected_vertices_3d.shape)}")
-        height, width = (int(v) for v in size)
-        out = rasterize_batch(projected_vertices_3d, self.faces, self.colors if pncc else None, height=height, width=width,
-                              depth=depth, tri_index=tri_index, negate_z=True, image_of_head=frame_of_head,
-                              num_images=num_frames, head_index=head_index)
-        if pncc:
-            out["pncc"] = out.pop("image")
-        return out
+        return self._render(projected_vertices_3d, size, pncc, depth=depth, tri_index=tri_index, image_of_head=frame_of_head,
+                            num_images=num_frames, head_index=head_index)
 
 
 # RenderPipeline's keyword arguments and defaults (Sim3DR/lighting.py:24-32)
@@ -359,25 +367,8 @@ def render_lit(vertices: torch.Tensor, triangles: torch.Tensor, *, height: int, 
     height, width = int(height), int(width)
     if height <= 0 or width <= 0 or height * width >= 1 << 31:
         raise ValueError(f"bad image size {height} x {width}")
-    mapped = image_of_head is not None
-    if mapped != (num_images is not None):
-        raise ValueError("image_of_head and num_images go together")
-    n_out = B
-    if mapped:
-        if image_of_head.shape != (B,) or image_of_head.dtype != torch.int32 or image_of_head.device != dev:
-            raise ValueError(f"image_of_head must be a [{B}] int32 tensor on the vertices' device")
-        n_out = int(num_images)
-        if n_out < 0:
-            raise ValueError(f"num_images must be >= 0, got {n_out}")
-        if B * ntri > 2 ** 32 - 2:
-            raise ValueError(f"{B} heads x {ntri} triangles exceed 2^32 - 2 (head, triangle) pairs")
-        image_of_head = image_of_head.contiguous()
-    if image is None:
-        out = torch.zeros(n_out, height, width, 3, dtype=torch.uint8, device=dev)
-    else:
-        if tuple(image.shape) != (n_out, height, width, 3) or image.dtype != torch.uint8:
-            raise ValueError(f"image must be [{n_out},{height},{width},3] uint8")
-        out = image.to(dev, copy=True).contiguous()
+    n_out, image_of_head = _image_map(image_of_head, num_images, B, ntri, dev)
+    out = _output_image(image, n_out, height, width, 3, dev)
     if B == 0 or n_out == 0:
         return out
     off, adj = _adjacency(triangles, nv)
@@ -387,7 +378,7 @@ def render_lit(vertices: torch.Tensor, triangles: torch.Tensor, *, height: int, 
     with torch.cuda.device(dev):
         _lib.check(lib.dad3d_render_lit(vertices.data_ptr(), nv, B, triangles.data_ptr(), ntri, off.data_ptr(),
                                         adj.data_ptr(), 1 if negate_z else 0, L,
-                                        image_of_head.data_ptr() if mapped else None, n_out, height, width,
+                                        image_of_head.data_ptr() if image_of_head is not None else None, n_out, height, width,
                                         light.data_ptr(), out.data_ptr(), key.data_ptr(),
                                         torch.cuda.current_stream(dev).cuda_stream), "dad3d_render_lit")
     return out
