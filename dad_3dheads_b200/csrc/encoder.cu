@@ -28,13 +28,27 @@ constexpr int kHeatCat = 128;      // heat-map slot inside the FusionLayer conca
 constexpr int kMlpOut = 549;       // 403 + 10 + 136
 constexpr float kLimitValue = 3.0f;
 
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+template <class T>
+using DevPtr = std::unique_ptr<T, CudaFree>;   // device memory, freed with its owner
+
+template <class T>
+bool upload(DevPtr<T>* d, const T* h, size_t n) {
+  void* p = nullptr;
+  if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) return false;
+  d->reset(static_cast<T*>(p));
+  return cudaMemcpy(p, h, n * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
+}
+
 struct ConvW {
   std::string name;
   int cout = 0, cin = 0, R = 1, S = 1;
   int cout_pad = 0, cin_pad = 0, block_n = 0;
-  uint16_t* d_w = nullptr;      // [P][cout_pad][R*S*cin_pad] bf16 pieces
-  float* d_bias = nullptr;      // [cout_pad]
-  float* d_scale = nullptr;     // [cout_pad] 2^-s per output channel (fp16 pieces: weights are stored as w * 2^s)
+  DevPtr<uint16_t> d_w;         // [P][cout_pad][R*S*cin_pad] bf16 pieces
+  DevPtr<float> d_bias;         // [cout_pad]
+  DevPtr<float> d_scale;        // [cout_pad] 2^-s per output channel (fp16 pieces: weights are stored as w * 2^s)
   CUtensorMap map_b[kMaxPieces];      // box 64 x block_n
   CUtensorMap map_b64[kMaxPieces];    // box 64 x 64 (small problems: more, narrower tiles to fill the SMs)
   bool has_b64 = false;
@@ -75,9 +89,29 @@ struct TensorInfo {
   uint8_t* ptr = nullptr;
   std::string name;                 // debug tag (layer that produced it)
   long long plane_elems() const { return static_cast<long long>(N) * H * W * C; }
+  // piece plane p lives at ptr + p * plane_elems(), NHWC
+  uint16_t* plane(int p) const { return reinterpret_cast<uint16_t*>(ptr) + static_cast<size_t>(p) * plane_elems(); }
+  ActView view(int fp16) const { return ActView{plane(0), plane_elems(), planes, C, fp16}; }
+  // 4-D (C, W, H, N) tensor map of plane p; box and element strides (nullptr: 1) as make_tmap_16bit takes them.  c_ext /
+  // w_ext (when non-zero) replace the two innermost extents while the strides stay those of the tensor: the stem reads
+  // overlapping 64-element windows that start at every 16-channel pixel.
+  bool nhwc_map(CUtensorMap* m, int p, const uint32_t* box, const uint32_t* es, int swizzle_bytes, uint64_t c_ext = 0,
+                uint64_t w_ext = 0) const {
+    const uint64_t dims[4] = {c_ext ? c_ext : static_cast<uint64_t>(C), w_ext ? w_ext : static_cast<uint64_t>(W),
+                              static_cast<uint64_t>(H), static_cast<uint64_t>(N)};
+    const uint64_t strides[3] = {static_cast<uint64_t>(C) * 2, static_cast<uint64_t>(W) * C * 2,
+                                 static_cast<uint64_t>(H) * W * C * 2};
+    return make_tmap_16bit(m, plane(p), 4, dims, strides, box, es, swizzle_bytes);
+  }
 };
 
 enum StepKind { kStemConv, kStemS2d, kStemPool, kConv, kFuse, kConcat, kGap, kFinalize, kHeatExport };
+
+// Step::res_mode, how Step::res enters a conv: residual add (on the K axis when the weights have identity columns), gate
+// multiply in the epilogue (FusionLayer), second 1x1 source (stride res_stride) whose weights are K-concatenated behind
+enum ResMode { kResNone = 0, kResAdd = 1, kResGate = 2, kResSource2 = 4 };
+// Step::variant: the step runs always, only when the caller asks for the heat-map, or only when it does not
+enum Variant { kAlways = 0, kWithHeatmap = 1, kWithoutHeatmap = 2 };
 
 struct Step {
   StepKind kind;
@@ -85,16 +119,16 @@ struct Step {
   int in = -1, out = -1, res = -1, out_f32 = -1, in2 = -1, in3 = -1;
   // conv
   const ConvW* w = nullptr;
-  int stride = 1, pad = 0, relu = 0, res_mode = 0, res_stride = 1;
+  int stride = 1, pad = 0, relu = 0, res_mode = kResNone, res_stride = 1;
   int up2 = 0;                  // output stored 2x nearest-up-sampled ([N, 2Ho, 2Wo, C])
   int parity = 0;               // 1 + 2a + b: 1x1 conv over the input pixels (2i + a, 2j + b) only, output stored to the same
                                 // pixels of the full-resolution tensor; the residual (res) lives on the half-resolution grid
-  int variant = 0;              // 0: always run; 1: only when the heat-map is requested; 2: only when it is not
+  int variant = kAlways;
   int sparse_rows = 0;          // heat-map head restricted to the output rows the FusionLayer's bilinear resampling reads
   int stem = 0;                 // the stem as a GEMM: input = space-to-depth image, A map = overlapping 4-pixel windows
-  GemmMaps maps;
-  GemmGeom geom;
-  EpiConv::Params epi;
+  GemmMaps maps{};
+  GemmGeom geom{};
+  EpiConv::Params epi{};
   // fuse
   float fw[3] = {0, 0, 0};
   int nsrc = 0;
@@ -109,6 +143,29 @@ struct Plan {
   int t_mlp_out = -1, t_heat = -1, t_c4 = -1;
 };
 
+// the DAD3D_* switches, read once at dad3d_encoder_create (DESIGN.md 4.4)
+struct Switches {
+  bool stem_simt = false;          // DAD3D_STEM_SIMT=1: run the stem on the fp32 CUDA-core kernel instead of the tile engine
+  bool halo = true;                // halo-reuse tiles for the 3x3 stride-1 layers (DAD3D_HALO=0 selects the per-tap path)
+  int halo_cluster = 1;            // DAD3D_HALO_CLUSTER=2: halo layers run as clusters of 2 row tiles that multicast the weights
+  bool td_parity = false;          // DAD3D_TD_PARITY=1: large top-down nodes as four parity launches
+  bool heat_sparse = true;         // DAD3D_HEAT_SPARSE=0: always compute the full heat-map
+  bool pdl = false;                // programmatic dependent launch for the tile-engine kernels (DAD3D_PDL=1 enables)
+};
+
+Switches read_switches() {
+  auto first = [](const char* name) { const char* e = std::getenv(name); return e ? e[0] : '\0'; };
+  Switches sw;
+  sw.pdl = first("DAD3D_PDL") == '1';
+  sw.halo = first("DAD3D_HALO") != '0';
+  sw.halo_cluster = first("DAD3D_HALO_CLUSTER") == '2' ? 2 : 1;
+  sw.td_parity = first("DAD3D_TD_PARITY") == '1';
+  const char* heat = std::getenv("DAD3D_HEAT_SPARSE");
+  sw.heat_sparse = !(heat && std::atoi(heat) == 0);
+  sw.stem_simt = first("DAD3D_STEM_SIMT") == '1';
+  return sw;
+}
+
 }  // namespace
 
 struct dad3d_encoder {
@@ -117,19 +174,14 @@ struct dad3d_encoder {
   int P = 3;                       // pieces per operand
   int fp16 = 0;                    // piece format: 0 = bf16 (1-3 pieces), 1 = fp16 hi/lo (per-channel scaled weights)
   std::map<std::string, ConvW> convs;
-  float* d_stem_w = nullptr;       // [147][64]
-  float* d_stem_b = nullptr;       // [64]
+  DevPtr<float> d_stem_w;          // [147][64]
+  DevPtr<float> d_stem_b;          // [64]
   float bifpn_w[2][20];            // per block: w1 normalised [2][4] then w2 normalised [3][4]
   std::unique_ptr<Plan> plan;
   size_t ws_cache_B = 0, ws_cache_bytes = 0;
-  bool stem_simt = false;          // env DAD3D_STEM_SIMT=1: run the stem on the fp32 CUDA-core kernel instead of the tile engine
-  bool use_halo = true;            // halo-reuse tiles for the 3x3 stride-1 layers (env DAD3D_HALO=0 selects the per-tap path)
-  int halo_cluster = 1;            // env DAD3D_HALO_CLUSTER=2: halo layers run as clusters of 2 row tiles that multicast the weights
+  Switches sw;
   GemmLaunchCache gemm_cache;      // the tile engine of this handle's operand format (the only one it launches)
   bool stem_configured = false;    // cudaFuncSetAttribute done on this handle's device
-  bool td_parity = false;          // env DAD3D_TD_PARITY=1: large top-down nodes as four parity launches
-  bool heat_sparse = true;         // env DAD3D_HEAT_SPARSE=0: always compute the full heat-map
-  bool use_pdl = false;            // programmatic dependent launch for the tile-engine kernels (env DAD3D_PDL=1 enables)
   bool debug_keep_all = false;     // disable buffer reuse so every activation can be read back after a forward
   // live profiling of the dominant kernel (bench.py roofline): CUDA events around every tile_gemm launch
   bool profile = false;
@@ -143,13 +195,30 @@ struct dad3d_encoder {
 namespace {
 
 // ---------------------------------------------------------------------------------------------- plan building
+// what a conv / linear layer step does besides reading its input; call sites name the fields they set
+struct ConvArgs {
+  int stride = 1, pad = 0;
+  bool relu = false;
+  int res = -1;                  // second tensor, entering as res_mode says
+  int res_mode = kResNone;
+  int res_stride = 1;            // kResSource2: stride of the second source
+  bool up2 = false;              // the output is written nearest-up-sampled by 2
+  bool f32_out = false;          // an fp32 output ...
+  bool pieces_out = true;        // ... and / or the piece planes
+  int* f32_id = nullptr;         // receives the fp32 output's tensor id
+  int reuse_f32 = -1;            // write the fp32 output into this tensor instead of a new one
+  int variant = kAlways;
+  bool sparse_rows = false;
+};
+
 struct Builder {
   dad3d_encoder* enc;
   Plan* plan;
   int B;
 
-  int tensor(int N, int H, int W, int C, bool f32 = false) {
+  int tensor(const std::string& name, int N, int H, int W, int C, bool f32 = false) {
     TensorInfo t;
+    t.name = name;
     t.N = N; t.H = H; t.W = W; t.C = C; t.f32 = f32;
     t.planes = f32 ? 1 : enc->P;
     t.bytes = align_up(static_cast<size_t>(t.plane_elems()) * (f32 ? 4 : 2) * t.planes, 1024);
@@ -172,35 +241,19 @@ struct Builder {
     auto it = enc->convs.find(name);
     return it == enc->convs.end() ? nullptr : &it->second;
   }
-  // conv / linear layer; returns the output tensor id (pieces) unless f32_only
-  // res_mode: 0 none, 1 residual add, 2 gate multiply, 4 second 1x1 source (stride res_stride) whose weights are
-  // K-concatenated behind the layer's own; up2: the output is written nearest-up-sampled by 2
-  int conv(const std::string& name, int in, int stride, int pad, bool relu, int res = -1, int res_mode = 0,
-           bool f32_out = false, bool pieces_out = true, int* f32_id = nullptr, int res_stride = 1, bool up2 = false,
-           int variant = 0, int reuse_f32 = -1, bool sparse_rows = false) {
+  // conv / linear layer; returns the output tensor id (pieces), -1 without piece output
+  int conv(const std::string& name, int in, const ConvArgs& a) {
     const ConvW* w = W(name);
     const TensorInfo ti = plan->tensors[in];
-    const int Ho = (ti.H + 2 * pad - w->R) / stride + 1;
-    const int Wo = (ti.W + 2 * pad - w->S) / stride + 1;
-    Step s;
-    std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kConv;
-    s.in = in;
-    s.w = w;
-    s.stride = stride;
-    s.pad = pad;
-    s.relu = relu ? 1 : 0;
-    s.res = res;
-    s.res_mode = res_mode;
-    s.res_stride = res_stride;
-    s.up2 = up2 ? 1 : 0;
-    s.out = pieces_out ? tensor(ti.N, up2 ? 2 * Ho : Ho, up2 ? 2 * Wo : Wo, w->cout_pad) : -1;
-    s.out_f32 = f32_out ? (reuse_f32 >= 0 ? reuse_f32 : tensor(ti.N, Ho, Wo, w->cout_pad, true)) : -1;
-    s.variant = variant;
-    s.sparse_rows = sparse_rows ? 1 : 0;
-    if (s.out >= 0) plan->tensors[s.out].name = name;
-    if (s.out_f32 >= 0) plan->tensors[s.out_f32].name = name + (pieces_out ? ".f32" : "");
-    if (f32_id) *f32_id = s.out_f32;
+    const int Ho = (ti.H + 2 * a.pad - w->R) / a.stride + 1;
+    const int Wo = (ti.W + 2 * a.pad - w->S) / a.stride + 1;
+    Step s{.kind = kConv, .in = in, .res = a.res, .w = w, .stride = a.stride, .pad = a.pad, .relu = a.relu,
+           .res_mode = a.res_mode, .res_stride = a.res_stride, .up2 = a.up2, .variant = a.variant,
+           .sparse_rows = a.sparse_rows};
+    s.out = a.pieces_out ? tensor(name, ti.N, a.up2 ? 2 * Ho : Ho, a.up2 ? 2 * Wo : Wo, w->cout_pad) : -1;
+    if (a.f32_out)
+      s.out_f32 = a.reuse_f32 >= 0 ? a.reuse_f32 : tensor(name + (a.pieces_out ? ".f32" : ""), ti.N, Ho, Wo, w->cout_pad, true);
+    if (a.f32_id) *a.f32_id = s.out_f32;
     push(s);
     return s.out;
   }
@@ -216,177 +269,134 @@ void pick_tile(int Wo, int Ho, int* tw, int* th, int* tn) {
   *tn = kBlockM / (w * h);
 }
 
+// ResNet-50 stage si over x (pytorchcv resnet50: stride on the first 1x1 of the first unit of stages 2..4)
+int res_stage(Builder& b, int si, int x) {
+  int cur = x;
+  for (int ui = 0; ui < kStageUnits[si]; ++ui) {
+    const std::string p = "s" + std::to_string(si + 1) + "u" + std::to_string(ui + 1);
+    const int stride = (ui == 0 && si != 0) ? 2 : 1;
+    int y = b.conv(p + "c1", cur, {.stride = stride, .relu = true});
+    y = b.conv(p + "c2", y, {.pad = 1, .relu = true});
+    if (ui == 0) {
+      // first unit of a stage: the projection shortcut (1x1, stride s, BN) is K-concatenated behind the last 1x1 --
+      // out = relu([W3 | Wid] [y ; x_strided] + b3 + bid): one GEMM, the shortcut tensor is never materialised
+      cur = b.conv(p + "c3", y, {.relu = true, .res = cur, .res_mode = kResSource2, .res_stride = stride});
+    } else {
+      cur = b.conv(p + "c3", y, {.relu = true, .res = cur, .res_mode = kResAdd});
+    }
+  }
+  return cur;
+}
+
+// one BiFPNBlock (bifpn.py:101-131) over the five levels feat[], which it replaces by its outputs
+void bifpn_block(Builder& b, int li, int feat[5]) {
+  Plan* plan = b.plan;
+  auto fuse = [&](int a, float wa, int s1, float w1, int s2, float w2) {
+    const TensorInfo ta = plan->tensors[a];
+    const int out = b.tensor("fuse" + std::to_string(plan->steps.size()), ta.N, ta.H, ta.W, ta.C);
+    b.push({.kind = kFuse, .in = a, .out = out, .in2 = s1, .in3 = s2, .fw = {wa, w1, w2}, .nsrc = s2 >= 0 ? 3 : 2});
+    return out;
+  };
+  // (w1 [2][4], the top-down fusion scalars, is folded into the weights on the host)
+  const float* w2 = &b.enc->bifpn_w[li][8];     // [3][4]
+  const std::string p = "b" + std::to_string(li) + "_";
+  const int p3x = feat[0], p4x = feat[1], p5x = feat[2], p6x = feat[3], p7x = feat[4];
+  const int p7td = p7x;
+  // top-down nodes (bifpn.py:111-114): node(w0*a + w1*up(b)) = relu(W0 a + up(W1 b) + shift); the fusion scalars are
+  // folded into the two weight sets on the host.  The low-resolution product is stored nearest-up-sampled (every pixel
+  // to its 2x2 block) and enters the node's GEMM through identity columns on the K axis, like a ResUnit residual.
+  // DAD3D_TD_PARITY=1, maps of >= 32 rows: the up-sampled branch is never materialised -- the node runs as four launches,
+  // one per pixel parity (a, b): a stride-2 view of the input starting at (a, b), the half-resolution product as the
+  // K-axis residual, and a store to the pixels (2i + a, 2j + b).  Measured slower than the default (one launch over the
+  // full map with the 4x-stored branch as residual: P3 node 222 -> 231 us, P4 73 -> 103 us), so it is opt-in.
+  auto td_node = [&](const std::string& name, int a, int lower) {
+    const TensorInfo ta = plan->tensors[a];
+    if (!b.enc->sw.td_parity || ta.H < 32) {
+      const int u = b.conv(name + "_u", lower, {.up2 = true});
+      return b.conv(name, a, {.relu = true, .res = u, .res_mode = kResAdd});
+    }
+    const int u = b.conv(name + "_u", lower, {});
+    const ConvW* w = b.W(name);
+    const int out = b.tensor(name, ta.N, ta.H, ta.W, w->cout_pad);
+    for (int ab = 0; ab < 4; ++ab)
+      b.push({.kind = kConv, .in = a, .out = out, .res = u, .w = w, .stride = 2, .relu = 1, .res_mode = kResAdd,
+              .parity = 1 + ab});
+    return out;
+  };
+  const int p6td = td_node(p + "p6td", p6x, p7td);
+  const int p5td = td_node(p + "p5td", p5x, p6td);
+  const int p4td = td_node(p + "p4td", p4x, p5td);
+  const int p3td = td_node(p + "p3td", p3x, p4td);
+  const int p3out = p3td;
+  const int p4out = b.conv(p + "p4out", fuse(p4x, w2[0], p4td, w2[4 + 0], p3out, w2[8 + 0]), {.relu = true});
+  const int p5out = b.conv(p + "p5out", fuse(p5x, w2[1], p5td, w2[4 + 1], p4out, w2[8 + 1]), {.relu = true});
+  const int p6out = b.conv(p + "p6out", fuse(p6x, w2[2], p6td, w2[4 + 2], p5out, w2[8 + 2]), {.relu = true});
+  const int p7out = b.conv(p + "p7out", fuse(p7x, w2[3], p7td, w2[4 + 3], p6out, w2[8 + 3]), {.relu = true});
+  feat[0] = p3out; feat[1] = p4out; feat[2] = p5out; feat[3] = p6out; feat[4] = p7out;
+}
+
 int build_graph(Builder& b) {
   const int B = b.B;
   Plan* plan = b.plan;
   // ---- stem: conv7x7/2 + BN + ReLU (fp32 SIMT) -> maxpool 3x3/2 -> pieces [B,64,64,64]
-  const int t_stem = b.tensor(B, kImg / 2, kImg / 2, 64, /*f32=*/b.enc->stem_simt);   // tensor-core stem: piece planes
-  if (b.enc->stem_simt) {
-    Step s; s.kind = kStemConv; s.out_f32 = t_stem; std::memset(&s.maps, 0, sizeof(s.maps));
-    b.push(s);
+  const int t_stem = b.tensor("stem_conv", B, kImg / 2, kImg / 2, 64, /*f32=*/b.enc->sw.stem_simt);   // tensor-core stem: piece planes
+  if (b.enc->sw.stem_simt) {
+    b.push({.kind = kStemConv, .out_f32 = t_stem});
   } else {
     // tensor-core stem: 2x2 space-to-depth (+ piece split) of the image, then a 4x4/1 conv over 12 channels whose four
     // horizontal taps form one 64-element K block (4 k-blocks, K = 256 of which 147 are non-zero)
-    const int t_s2d = b.tensor(B, kImg / 2, kImg / 2 + kS2dPadW, 16);
-    plan->tensors[t_s2d].name = "s2d";
-    {
-      Step s; s.kind = kStemS2d; s.out = t_s2d; std::memset(&s.maps, 0, sizeof(s.maps));
-      b.push(s);
-    }
-    Step s;
-    std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kConv;
-    s.in = t_s2d;
-    s.w = b.W("stem");
-    s.stem = 1;
-    s.relu = 1;
-    s.out = t_stem;
-    b.push(s);
+    const int t_s2d = b.tensor("s2d", B, kImg / 2, kImg / 2 + kS2dPadW, 16);
+    b.push({.kind = kStemS2d, .out = t_s2d});
+    b.push({.kind = kConv, .in = t_s2d, .out = t_stem, .w = b.W("stem"), .relu = 1, .stem = 1});
   }
-  plan->tensors[t_stem].name = "stem_conv";
-  int x = b.tensor(B, kImg / 4, kImg / 4, 64);
-  plan->tensors[x].name = "stem";
-  {
-    Step s; s.kind = kStemPool; s.in = t_stem; s.out = x; std::memset(&s.maps, 0, sizeof(s.maps));
-    b.push(s);
-  }
-  // ---- ResNet-50 stages (pytorchcv resnet50: stride on the first 1x1 of the first unit of stages 2..4)
+  int x = b.tensor("stem", B, kImg / 4, kImg / 4, 64);
+  b.push({.kind = kStemPool, .in = t_stem, .out = x});
+  // ---- ResNet-50 stages 1..3
   int c_out[4] = {-1, -1, -1, -1};
-  auto run_stage = [&](int si, int xin) {
-    int cur = xin;
-    for (int ui = 0; ui < kStageUnits[si]; ++ui) {
-      const std::string p = "s" + std::to_string(si + 1) + "u" + std::to_string(ui + 1);
-      const int stride = (ui == 0 && si != 0) ? 2 : 1;
-      int y = b.conv(p + "c1", cur, stride, 0, true);
-      y = b.conv(p + "c2", y, 1, 1, true);
-      if (ui == 0) {
-        // first unit of a stage: the projection shortcut (1x1, stride s, BN) is K-concatenated behind the last 1x1 --
-        // out = relu([W3 | Wid] [y ; x_strided] + b3 + bid): one GEMM, the shortcut tensor is never materialised
-        cur = b.conv(p + "c3", y, 1, 0, true, cur, 4, false, true, nullptr, stride);
-      } else {
-        cur = b.conv(p + "c3", y, 1, 0, true, cur, 1);
-      }
-    }
-    return cur;
-  };
   for (int si = 0; si < 3; ++si) {
-    x = run_stage(si, x);
+    x = res_stage(b, si, x);
     c_out[si] = x;
   }
   const int c2 = c_out[0], c3 = c_out[1], c4 = c_out[2];
   // ---- BiFPN laterals (bifpn.py:137-145, 152-161)
   int feat[5];
   // P3's lateral conv is normally composed into b0_p3td on the host (its only consumer); a "lat3" record keeps it separate
-  feat[0] = b.W("lat3") ? b.conv("lat3", c2, 1, 0, false) : c2;
-  feat[1] = b.conv("lat4", c3, 1, 0, false);
-  feat[2] = b.conv("lat5", c4, 1, 0, false);
-  feat[3] = b.conv("lat6", c4, 2, 1, false);
-  feat[4] = b.conv("lat7", feat[3], 2, 1, true);
-  // ---- 2 x BiFPNBlock (bifpn.py:101-131)
-  auto fuse = [&](int a, float wa, int s1, float w1, int s2, float w2) {
-    const TensorInfo ta = plan->tensors[a];
-    Step s; std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kFuse;
-    s.in = a; s.in2 = s1; s.in3 = s2;
-    s.nsrc = s2 >= 0 ? 3 : 2;
-    s.fw[0] = wa; s.fw[1] = w1; s.fw[2] = w2;
-    s.out = b.tensor(ta.N, ta.H, ta.W, ta.C);
-    plan->tensors[s.out].name = "fuse" + std::to_string(plan->steps.size());
-    b.push(s);
-    return s.out;
-  };
-  for (int li = 0; li < 2; ++li) {
-    // (w1 [2][4], the top-down fusion scalars, is folded into the weights on the host)
-    const float* w2 = &b.enc->bifpn_w[li][8];     // [3][4]
-    const std::string p = "b" + std::to_string(li) + "_";
-    const int p3x = feat[0], p4x = feat[1], p5x = feat[2], p6x = feat[3], p7x = feat[4];
-    const int p7td = p7x;
-    // top-down nodes (bifpn.py:111-114): node(w0*a + w1*up(b)) = relu(W0 a + up(W1 b) + shift); the fusion scalars are
-    // folded into the two weight sets on the host.  The low-resolution product is stored nearest-up-sampled (every pixel
-    // to its 2x2 block) and enters the node's GEMM through identity columns on the K axis, like a ResUnit residual.
-    // DAD3D_TD_PARITY=1, maps of >= 32 rows: the up-sampled branch is never materialised -- the node runs as four launches,
-    // one per pixel parity (a, b): a stride-2 view of the input starting at (a, b), the half-resolution product as the
-    // K-axis residual, and a store to the pixels (2i + a, 2j + b).  Measured slower than the default (one launch over the
-    // full map with the 4x-stored branch as residual: P3 node 222 -> 231 us, P4 73 -> 103 us), so it is opt-in.
-    auto td_node = [&](const std::string& name, int a, int lower) {
-      const TensorInfo ta = plan->tensors[a];
-      if (!b.enc->td_parity || ta.H < 32) {
-        const int u = b.conv(name + "_u", lower, 1, 0, false, -1, 0, false, true, nullptr, 1, /*up2=*/true);
-        return b.conv(name, a, 1, 0, true, u, 1);
-      }
-      const int u = b.conv(name + "_u", lower, 1, 0, false);
-      const ConvW* w = b.W(name);
-      const int out = b.tensor(ta.N, ta.H, ta.W, w->cout_pad);
-      plan->tensors[out].name = name;
-      for (int ab = 0; ab < 4; ++ab) {
-        Step s;
-        std::memset(&s.maps, 0, sizeof(s.maps));
-        s.kind = kConv;
-        s.in = a; s.w = w; s.stride = 2; s.pad = 0; s.relu = 1;
-        s.res = u; s.res_mode = 1;
-        s.out = out;
-        s.parity = 1 + ab;
-        b.push(s);
-      }
-      return out;
-    };
-    const int p6td = td_node(p + "p6td", p6x, p7td);
-    const int p5td = td_node(p + "p5td", p5x, p6td);
-    const int p4td = td_node(p + "p4td", p4x, p5td);
-    const int p3td = td_node(p + "p3td", p3x, p4td);
-    const int p3out = p3td;
-    const int p4out = b.conv(p + "p4out", fuse(p4x, w2[0], p4td, w2[4 + 0], p3out, w2[8 + 0]), 1, 0, true);
-    const int p5out = b.conv(p + "p5out", fuse(p5x, w2[1], p5td, w2[4 + 1], p4out, w2[8 + 1]), 1, 0, true);
-    const int p6out = b.conv(p + "p6out", fuse(p6x, w2[2], p6td, w2[4 + 2], p5out, w2[8 + 2]), 1, 0, true);
-    const int p7out = b.conv(p + "p7out", fuse(p7x, w2[3], p7td, w2[4 + 3], p6out, w2[8 + 3]), 1, 0, true);
-    feat[0] = p3out; feat[1] = p4out; feat[2] = p5out; feat[3] = p6out; feat[4] = p7out;
-  }
+  feat[0] = b.W("lat3") ? b.conv("lat3", c2, {}) : c2;
+  feat[1] = b.conv("lat4", c3, {});
+  feat[2] = b.conv("lat5", c4, {});
+  feat[3] = b.conv("lat6", c4, {.stride = 2, .pad = 1});
+  feat[4] = b.conv("lat7", feat[3], {.stride = 2, .pad = 1, .relu = true});
+  for (int li = 0; li < 2; ++li) bifpn_block(b, li, feat);
   // ---- heat-map head (flame_regression.py:22-25): 3x3 conv 256 -> 68 (+bias), kept in fp32
   int t_heat = -1;
   // Two variants of the same layer: the full 64 x 64 map when the caller asks for the heat-map, otherwise only the output
   // rows that FusionLayer's align_corners bilinear 64 -> 16 resampling reads (31 of 64: the rows floor(i * 63 / 15) and the
   // next one) -- env DAD3D_HEAT_SPARSE=0 keeps the full map always.
-  const bool heat_sparse = b.enc->heat_sparse;
-  b.conv("heat", feat[0], 1, 1, false, -1, 0, /*f32_out=*/true, /*pieces_out=*/false, &t_heat, 1, false, heat_sparse ? 1 : 0);
+  const bool heat_sparse = b.enc->sw.heat_sparse;
+  b.conv("heat", feat[0], {.pad = 1, .f32_out = true, .pieces_out = false, .f32_id = &t_heat,
+                           .variant = heat_sparse ? kWithHeatmap : kAlways});
   if (heat_sparse)
-    b.conv("heat", feat[0], 1, 1, false, -1, 0, /*f32_out=*/true, /*pieces_out=*/false, nullptr, 1, false, 2, t_heat, true);
+    b.conv("heat", feat[0], {.pad = 1, .f32_out = true, .pieces_out = false, .reuse_f32 = t_heat,
+                             .variant = kWithoutHeatmap, .sparse_rows = true});
   plan->t_heat = t_heat;
   // ---- FusionLayer (flame_regression.py:33-42)
   plan->t_c4 = c4;
   const TensorInfo tc4 = plan->tensors[c4];
-  const int t_cat = b.tensor(B, tc4.H, tc4.W, 1024 + kHeatCat + kNumFilters);
-  plan->tensors[t_cat].name = "cat";
-  {
-    Step s; std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kConcat; s.in = c4; s.in2 = t_heat; s.in3 = feat[2]; s.out = t_cat;
-    b.push(s);
-  }
-  x = b.conv("fusion", t_cat, 1, 0, false, c4, 2);
+  const int t_cat = b.tensor("cat", B, tc4.H, tc4.W, 1024 + kHeatCat + kNumFilters);
+  b.push({.kind = kConcat, .in = c4, .out = t_cat, .in2 = t_heat, .in3 = feat[2]});
+  x = b.conv("fusion", t_cat, {.res = c4, .res_mode = kResGate});
   // ---- stage 4
-  x = run_stage(3, x);
+  x = res_stage(b, 3, x);
   // ---- heads (flame_regression.py:45-59, 96-106): GAP -> [3 x Linear 2048->512 + ReLU] -> block-diagonal second layers
   const TensorInfo tx = plan->tensors[x];
-  const int t_gap = b.tensor(1, 1, B, tx.C);
-  plan->tensors[t_gap].name = "gap";
-  {
-    Step s; std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kGap; s.in = x; s.out = t_gap;
-    b.push(s);
-  }
-  const int t_h = b.conv("mlp1", t_gap, 1, 0, true);
+  const int t_gap = b.tensor("gap", 1, 1, B, tx.C);
+  b.push({.kind = kGap, .in = x, .out = t_gap});
+  const int t_h = b.conv("mlp1", t_gap, {.relu = true});
   int t_out = -1;
-  b.conv("mlp2", t_h, 1, 0, false, -1, 0, true, false, &t_out);
+  b.conv("mlp2", t_h, {.f32_out = true, .pieces_out = false, .f32_id = &t_out});
   plan->t_mlp_out = t_out;
-  {
-    Step s; std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kFinalize; s.in = t_out;
-    b.push(s);
-  }
-  {
-    Step s; std::memset(&s.maps, 0, sizeof(s.maps));
-    s.kind = kHeatExport; s.in = t_heat;
-    b.push(s);
-  }
+  b.push({.kind = kFinalize, .in = t_out});
+  b.push({.kind = kHeatExport, .in = t_heat});
   return DAD3D_OK;
 }
 
@@ -422,6 +432,199 @@ size_t assign_offsets(std::vector<TensorInfo>& ts) {
   return total;
 }
 
+// the residual rides the K axis: through the weights' identity columns, or as a second 1x1 source
+bool res_identity(const Step& s) { return s.res >= 0 && s.res_mode == kResAdd && s.w->has_identity; }
+bool res_source2(const Step& s) { return s.res >= 0 && s.res_mode == kResSource2; }
+
+// the operand ring of this handle's pieces at width block_n, before a tile is chosen: asks what shared memory fits
+GemmGeom ring_probe(int P, int block_n, int frag_epi) {
+  GemmGeom g{};
+  g.nA = P; g.nB = P; g.block_n = block_n; g.frag_epi = frag_epi;
+  return g;
+}
+
+// Every launch decision of one conv step, from shapes and the handle's switches (no pointers), and the checks on them.
+// Written in the order of tests/pingpong_model.py::geometry, which restates it for the CPU tests: change both together.
+int conv_geometry(const dad3d_encoder* enc, const Plan& plan, const Step& s, GemmGeom* out) {
+  const TensorInfo& ti = plan.tensors[s.in];
+  const ConvW* w = s.w;
+  const int P = enc->P;
+  const bool res_in_k = res_identity(s), src2 = res_source2(s);
+  const int cin2 = src2 ? plan.tensors[s.res].C : 0;
+  if (!s.stem && ti.C + cin2 != w->cin_pad) {
+    set_error("layer " + w->name + ": input has " + std::to_string(ti.C) + "+" + std::to_string(cin2) +
+              " channels, weights expect " + std::to_string(w->cin_pad));
+    return DAD3D_ERR_INVALID;
+  }
+  GemmGeom g{};
+  const int Ho = s.stem ? ti.H : s.parity ? ti.H / 2 : (ti.H + 2 * s.pad - w->R) / s.stride + 1;
+  const int Wo = s.stem ? ti.W - kS2dPadW : s.parity ? ti.W / 2 : (ti.W + 2 * s.pad - w->S) / s.stride + 1;
+  g.Wo = Wo; g.Ho = Ho; g.Nimg = ti.N;
+  g.stride = s.stride;
+  g.R = w->R; g.S = w->S; g.pad_h = s.pad; g.pad_w = s.pad;
+  if (s.stem) { g.pad_h = 2; g.pad_w = 0; }                                             // 4 vertical taps
+  if (s.parity) { g.pad_h = -((s.parity - 1) >> 1); g.pad_w = -((s.parity - 1) & 1); }   // input pixel (2i + a, 2j + b)
+  g.cl_m = 1; g.cl_n = 1;
+  g.frag_epi = s.out >= 0 ? 1 : 0;                  // piece outputs: fragment epilogue, no shared-memory accumulator tile
+  pick_tile(Wo, Ho, &g.tw, &g.th, &g.tn);
+  // 3x3 / stride 1 / pad 1 layers: 8 x 16-pixel tiles whose nine taps share one halo patch in shared memory (tile_gemm.cuh
+  // "halo mode"); needs a map of at least 8 x 16 pixels and room for two halo patches + a two-deep weights ring (bf16x3
+  // at N = 128 has none).  The sparse heat rows use row-pair tiles (2 rows x 64 columns) through the per-tap path.
+  const bool halo = enc->sw.halo && !s.stem && w->R == 3 && w->S == 3 && s.stride == 1 && s.pad == 1 &&
+                    Wo >= kHaloTW && Ho >= kHaloTH && gemm_halo_b_stages(ring_probe(P, w->block_n, g.frag_epi)) >= 2 &&
+                    !s.sparse_rows;
+  if (halo) { g.tw = kHaloTW; g.th = kHaloTH; g.tn = 1; }
+  g.tiles_w = ceil_div(Wo, g.tw);
+  g.tiles_h = ceil_div(Ho, g.th);
+  if (s.sparse_rows) {
+    // FusionLayer: F.interpolate(heatmap, size=(16, 16), mode="bilinear", align_corners=True) reads source rows
+    // y0 = floor(i * (Ho - 1) / 15) and min(y0 + 1, Ho - 1), i = 0..15 (flame_regression.py:33-41)
+    g.tw = Wo; g.th = 2; g.tn = 1;
+    if (g.tw * g.th != kBlockM) { set_error("sparse heat rows need a 64-pixel-wide map"); return DAD3D_ERR_INVALID; }
+    g.tiles_w = 1;
+    const int Hd = plan.tensors[plan.t_c4].H;        // the FusionLayer's target height (16)
+    g.rowmap_n = 0;
+    for (int i = 0; i < Hd && g.rowmap_n < 32; ++i) {
+      const float fy = (Hd > 1) ? i * (static_cast<float>(Ho - 1) / static_cast<float>(Hd - 1)) : 0.f;   // as fusion_concat_kernel
+      const int y0 = static_cast<int>(fy);
+      if (g.rowmap_n == 0 || g.rowmap[g.rowmap_n - 1] != y0) g.rowmap[g.rowmap_n++] = static_cast<unsigned char>(y0);
+    }
+    g.tiles_h = g.rowmap_n;
+  }
+  g.tiles_n = ceil_div(ti.N, g.tn);
+  // few row tiles (small maps / small batch): halve the tile width so that twice as many CTAs share the work; the
+  // full-width tile also needs a two-deep operand ring in shared memory
+  const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
+  const bool narrow = w->has_b64 && (m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms ||
+                                     gemm_max_stages(ring_probe(P, w->block_n, g.frag_epi)) < 2);
+  g.cin_blocks = s.stem ? 1 : ti.C / kBlockK;       // main source (the stem: one 64-element window); a second source adds
+  gemm_products(g, P);                              // res_kb blocks below
+  // ping-pong consumers (tile_gemm.cuh) on 128 x 64 tiles: fragment-epilogue launches outside halo mode (and so outside
+  // clusters) whose 64-wide ring is at least two deep, with more than one product per k-block and at most
+  // kPingPongMaxKb k-blocks per tile.  Measured on H100 (profiles/README.md): in fp16x2 at batch 64 every such launch of
+  // up to 32 k-blocks ran faster or level, the 3x3 layers of 36 and 72 k-blocks slower; with one product per k-block
+  // (bf16, batch 512) ping-pong everywhere was slower, its main loop being bound by the operand bytes that 64-wide
+  // tiles raise.
+  constexpr int kPingPongMaxKb = 32;
+  const int kb64 = w->R * w->S * g.cin_blocks + (res_in_k ? 1 : src2 ? cin2 / kBlockK : 0);   // k-blocks at block_n 64
+  g.pingpong = g.frag_epi && !halo && (w->block_n == 64 || w->has_b64) &&
+               gemm_max_stages(ring_probe(P, 64, g.frag_epi)) >= 2 && g.n_mma > 1 && kb64 <= kPingPongMaxKb ? 1 : 0;
+  g.block_n = narrow || g.pingpong ? 64 : w->block_n;
+  g.n_tiles = w->cout_pad / g.block_n;
+  if (res_in_k) {                                   // "+ identity(x)" performed by the tensor core
+    g.res_kb = g.block_n / kBlockK;
+    g.n_mma_res = P;
+    for (int i = 0; i < P; ++i) {
+      g.mma_res_a[i] = P - 1 - i;                   // smallest piece first
+      g.mma_res_acc[i] = (g.n_acc == 2 && g.mma_res_a[i] != 0) ? 1 : 0;
+    }
+  }
+  if (src2) {                                       // projection shortcut as a second K segment
+    g.res_kb = cin2 / kBlockK;
+    g.res_kind = 1;
+    g.res_stride = s.res_stride;
+  }
+  g.stages = gemm_max_stages(g);
+  if (halo) {
+    g.halo = 1;
+    if (enc->sw.halo_cluster == 2 && g.block_n == 128 && w->has_b64 && m_tiles >= 2 * enc->num_sms) {
+      g.cl_m = 2;                                   // two row tiles share every weight tile (each loads half, multicast)
+      g.sched = 1;
+    }
+    g.stages = 2;
+    g.stages_b = gemm_halo_b_stages(g);
+    if (g.stages_b < 2) { set_error("layer " + w->name + ": halo pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
+  }
+  // (the 80 / 96-wide heads at three pieces fit one operand stage only: the producer then refills behind each k-block)
+  if (g.stages < 1) { set_error("layer " + w->name + ": pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
+  if (s.res >= 0 && !src2 && plan.tensors[s.res].C != w->cout_pad) {
+    set_error("layer " + w->name + ": residual channel mismatch");
+    return DAD3D_ERR_INVALID;
+  }
+  if (s.out >= 0 && g.block_n != 64 && g.block_n != 128) {
+    set_error("layer " + w->name + ": piece outputs need block_n 64 or 128");
+    return DAD3D_ERR_INVALID;
+  }
+  *out = g;
+  return DAD3D_OK;
+}
+
+// the tensor maps of one conv step (after conv_geometry): input pieces, weight pieces, residual / second source, outputs
+int conv_maps(const dad3d_encoder* enc, const Plan& plan, Step& s) {
+  const GemmGeom& g = s.geom;
+  const TensorInfo& ti = plan.tensors[s.in];
+  const ConvW* w = s.w;
+  {
+    // stem: row x of the A operand is the 64-element window that starts at padded s2d pixel x (dim 1 advances by one
+    // 16-channel pixel = 32 bytes while the window is 128 bytes long: consecutive rows overlap)
+    const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(g.halo ? kHaloPW : g.tw * s.stride),
+                             static_cast<uint32_t>(g.halo ? kHaloPH : g.th * s.stride), static_cast<uint32_t>(g.tn)};
+    const uint32_t es[4] = {1, static_cast<uint32_t>(s.stride), static_cast<uint32_t>(s.stride), 1};
+    for (int p = 0; p < enc->P; ++p) {
+      if (!ti.nhwc_map(&s.maps.a[p], p, box, es, 128, s.stem ? kBlockK : 0, s.stem ? g.Wo : 0)) return DAD3D_ERR_CUDA;
+      s.maps.b[p] = (g.block_n != w->block_n || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];
+    }
+  }
+  if (res_identity(s) || res_source2(s)) {
+    const TensorInfo& tr = plan.tensors[s.res];
+    const int rs = res_source2(s) ? s.res_stride : 1;
+    const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(g.tw * rs), static_cast<uint32_t>(g.th * rs),
+                             static_cast<uint32_t>(g.tn)};
+    const uint32_t es[4] = {1, static_cast<uint32_t>(rs), static_cast<uint32_t>(rs), 1};
+    for (int p = 0; p < enc->P; ++p)
+      if (!tr.nhwc_map(&s.maps.r[p], p, box, es, 128)) return DAD3D_ERR_CUDA;
+  }
+  if (s.out < 0) return DAD3D_OK;
+  const TensorInfo& to = plan.tensors[s.out];
+  // per-warp store box: 16 consecutive tile rows = (bw x bh x bn) output pixels x 32 channels (SWIZZLE_64B rows)
+  const int nc = 32;
+  const int bw = std::min(g.tw, 16);
+  const int bh = std::min(g.th, 16 / bw);
+  const int bn = 16 / (bw * bh);
+  if (s.up2 || s.parity) {
+    // [N, 2Ho, 2Wo, C] seen as (C, b, j, a, n*Ho + i): pixel (2i + a, 2j + b); a box with b = a = 1 addresses the
+    // sub-grid of one parity, so the same staging tile is stored four times
+    const uint64_t C2 = static_cast<uint64_t>(to.C) * 2;
+    const uint64_t dims[5] = {static_cast<uint64_t>(to.C), 2, static_cast<uint64_t>(g.Wo), 2,
+                              static_cast<uint64_t>(to.N) * g.Ho};
+    const uint64_t strides[4] = {C2, 2 * C2, static_cast<uint64_t>(to.W) * C2, 2 * static_cast<uint64_t>(to.W) * C2};
+    const uint32_t box[5] = {static_cast<uint32_t>(nc), 1, static_cast<uint32_t>(bw), 1, static_cast<uint32_t>(bh * bn)};
+    for (int p = 0; p < to.planes; ++p)
+      if (!make_tmap_16bit(&s.maps.c[p], to.plane(p), 5, dims, strides, box, nullptr, nc * 2)) return DAD3D_ERR_CUDA;
+    return DAD3D_OK;
+  }
+  const uint32_t box[4] = {static_cast<uint32_t>(nc), static_cast<uint32_t>(bw), static_cast<uint32_t>(bh),
+                           static_cast<uint32_t>(bn)};
+  for (int p = 0; p < to.planes; ++p)
+    if (!to.nhwc_map(&s.maps.c[p], p, box, nullptr, nc * 2)) return DAD3D_ERR_CUDA;
+  return DAD3D_OK;
+}
+
+// the epilogue parameters of one conv step
+void conv_epilogue(const dad3d_encoder* enc, const Plan& plan, Step& s) {
+  EpiConv::Params& ep = s.epi;
+  ep.bias = s.w->d_bias.get();
+  ep.scale = s.w->d_scale.get();
+  ep.relu = s.relu;
+  ep.res_mode = (res_identity(s) || res_source2(s)) ? kResNone : s.res_mode;   // a K-axis residual is in the product
+  ep.res = s.res >= 0 ? plan.tensors[s.res].view(enc->fp16) : ActView{nullptr, 0, 0, 0, enc->fp16};
+  ep.up2 = s.up2;
+  ep.parity = s.parity;
+  if (s.out >= 0) {
+    const TensorInfo& to = plan.tensors[s.out];
+    ep.out = to.plane(0);
+    ep.out_plane = to.plane_elems();
+    ep.out_planes = to.planes;
+    ep.ld_out = to.C;
+  }
+  if (s.out_f32 >= 0) {
+    const TensorInfo& to = plan.tensors[s.out_f32];
+    ep.out_f32 = reinterpret_cast<float*>(to.ptr);
+    ep.ld_f32 = to.C;
+  }
+}
+
+// the plan of one batch size: the step graph, tensor lifetimes and workspace offsets, then every conv step's launch
 int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_only, size_t* need) {
   std::unique_ptr<Plan> plan(new Plan());
   plan->B = B;
@@ -441,203 +644,11 @@ int make_plan(dad3d_encoder* enc, int B, void* ws, size_t ws_bytes, bool layout_
   for (auto& t : plan->tensors) t.ptr = base + t.off;
   plan->ws = ws;
   plan->ws_bytes = ws_bytes;
-
-  auto view = [&](int id) {
-    ActView v{nullptr, 0, 0, 0, enc->fp16};
-    if (id < 0) return v;
-    const TensorInfo& t = plan->tensors[id];
-    v.base = reinterpret_cast<const uint16_t*>(t.ptr);
-    v.plane = t.plane_elems();
-    v.planes = t.planes;
-    v.C = t.C;
-    return v;
-  };
   for (Step& s : plan->steps) {
     if (s.kind != kConv) continue;
-    const TensorInfo& ti = plan->tensors[s.in];
-    const ConvW* w = s.w;
-    const bool src2 = s.res >= 0 && s.res_mode == 4;
-    const int cin2 = src2 ? plan->tensors[s.res].C : 0;
-    if (!s.stem && ti.C + cin2 != w->cin_pad) {
-      set_error("layer " + w->name + ": input has " + std::to_string(ti.C) + "+" + std::to_string(cin2) +
-                " channels, weights expect " + std::to_string(w->cin_pad));
-      return DAD3D_ERR_INVALID;
-    }
-    const int Ho = s.stem ? ti.H : s.parity ? ti.H / 2 : (ti.H + 2 * s.pad - w->R) / s.stride + 1;
-    const int Wo = s.stem ? ti.W - kS2dPadW : s.parity ? ti.W / 2 : (ti.W + 2 * s.pad - w->S) / s.stride + 1;
-    GemmGeom& g = s.geom;
-    std::memset(&g, 0, sizeof(g));
-    g.frag_epi = s.out >= 0 ? 1 : 0;                  // piece outputs: fragment epilogue, no shared-memory accumulator tile
-    pick_tile(Wo, Ho, &g.tw, &g.th, &g.tn);
-    // 3x3 / stride 1 / pad 1 layers: 8 x 16-pixel tiles whose nine taps share one halo patch in shared memory (tile_gemm.cuh
-    // "halo mode"); needs a map of at least 8 x 16 pixels and room for a two-deep weights ring (checked below)
-    bool halo = enc->use_halo && !s.stem && w->R == 3 && w->S == 3 && s.stride == 1 && s.pad == 1 && Wo >= kHaloTW &&
-                Ho >= kHaloTH;
-    if (halo) {                                       // two halo patches + at least two weight tiles must fit (bf16x3 at N = 128 does not)
-      GemmGeom probe;
-      std::memset(&probe, 0, sizeof(probe));
-      probe.nA = enc->P; probe.nB = enc->P; probe.block_n = w->block_n; probe.frag_epi = g.frag_epi;
-      halo = gemm_halo_b_stages(probe) >= 2;
-    }
-    if (s.sparse_rows) halo = false;                  // row-pair tiles (2 rows x 64 columns) through the per-tap path
-    if (halo) { g.tw = kHaloTW; g.th = kHaloTH; g.tn = 1; }
-    g.tiles_w = ceil_div(Wo, g.tw);
-    g.tiles_h = ceil_div(Ho, g.th);
-    if (s.sparse_rows) {
-      // FusionLayer: F.interpolate(heatmap, size=(16, 16), mode="bilinear", align_corners=True) reads source rows
-      // y0 = floor(i * (Ho - 1) / 15) and min(y0 + 1, Ho - 1), i = 0..15 (flame_regression.py:33-41)
-      g.tw = Wo; g.th = 2; g.tn = 1;
-      if (g.tw * g.th != kBlockM) { set_error("sparse heat rows need a 64-pixel-wide map"); return DAD3D_ERR_INVALID; }
-      g.tiles_w = 1;
-      const int Hd = plan->tensors[plan->t_c4].H;      // the FusionLayer's target height (16)
-      g.rowmap_n = 0;
-      for (int i = 0; i < Hd && g.rowmap_n < 32; ++i) {
-        const float fy = (Hd > 1) ? i * (static_cast<float>(Ho - 1) / static_cast<float>(Hd - 1)) : 0.f;   // as fusion_concat_kernel
-        const int y0 = static_cast<int>(fy);
-        if (g.rowmap_n == 0 || g.rowmap[g.rowmap_n - 1] != y0) g.rowmap[g.rowmap_n++] = static_cast<unsigned char>(y0);
-      }
-      g.tiles_h = g.rowmap_n;
-    }
-    g.tiles_n = ceil_div(ti.N, g.tn);
-    g.Wo = Wo; g.Ho = Ho; g.Nimg = ti.N;
-    g.stride = s.stride;
-    g.R = w->R; g.S = w->S; g.pad_h = s.pad; g.pad_w = s.pad;
-    g.cin_blocks = ti.C / kBlockK;                    // main source; a second source adds res_kb blocks below
-    if (s.stem) { g.cin_blocks = 1; g.pad_h = 2; g.pad_w = 0; }   // 4 vertical taps x one 64-element window
-    if (s.parity) { g.pad_h = -((s.parity - 1) >> 1); g.pad_w = -((s.parity - 1) & 1); }   // input pixel (2i + a, 2j + b)
-    g.cl_m = 1; g.cl_n = 1;
-    gemm_products(g, enc->P);
-    const bool res_in_k = s.res >= 0 && s.res_mode == 1 && w->has_identity;
-    // few row tiles (small maps / small batch): halve the tile width so that twice as many CTAs share the work
-    const int m_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
-    GemmGeom fit;                                     // the full-width tile needs a two-deep operand ring in shared memory
-    std::memset(&fit, 0, sizeof(fit));
-    fit.nA = enc->P; fit.nB = enc->P; fit.block_n = w->block_n; fit.frag_epi = g.frag_epi;
-    const bool narrow = w->has_b64 && (m_tiles * (w->cout_pad / w->block_n) * 2 <= enc->num_sms || gemm_max_stages(fit) < 2);
-    // ping-pong consumers (tile_gemm.cuh) on 128 x 64 tiles: fragment-epilogue launches outside halo mode (and so outside
-    // clusters) whose 64-wide ring is at least two deep, with more than one product per k-block and at most
-    // kPingPongMaxKb k-blocks per tile.  Measured on H100 (profiles/README.md): in fp16x2 at batch 64 every such launch of
-    // up to 32 k-blocks ran faster or level, the 3x3 layers of 36 and 72 k-blocks slower; with one product per k-block
-    // (bf16, batch 512) ping-pong everywhere was slower, its main loop being bound by the operand bytes that 64-wide
-    // tiles raise.
-    constexpr int kPingPongMaxKb = 32;
-    const int kb64 = w->R * w->S * g.cin_blocks + (res_in_k ? 1 : src2 ? cin2 / kBlockK : 0);   // k-blocks at block_n 64
-    fit.block_n = 64;
-    g.pingpong = g.frag_epi && !halo && (w->block_n == 64 || w->has_b64) && gemm_max_stages(fit) >= 2 &&
-                 g.n_mma > 1 && kb64 <= kPingPongMaxKb ? 1 : 0;
-    const int block_n = narrow || g.pingpong ? 64 : w->block_n;
-    g.block_n = block_n;
-    g.n_tiles = w->cout_pad / block_n;
-    if (res_in_k) {                                   // "+ identity(x)" performed by the tensor core
-      g.res_kb = block_n / kBlockK;
-      g.n_mma_res = enc->P;
-      for (int i = 0; i < enc->P; ++i) {
-        g.mma_res_a[i] = enc->P - 1 - i;              // smallest piece first
-        g.mma_res_acc[i] = (g.n_acc == 2 && g.mma_res_a[i] != 0) ? 1 : 0;
-      }
-    }
-    if (src2) {                                       // projection shortcut as a second K segment
-      g.res_kb = cin2 / kBlockK;
-      g.res_kind = 1;
-      g.res_stride = s.res_stride;
-    }
-    g.stages = gemm_max_stages(g);
-    if (halo) {
-      g.halo = 1;
-      if (enc->halo_cluster == 2 && block_n == 128 && w->has_b64 && m_tiles >= 2 * enc->num_sms) {
-        g.cl_m = 2;                                   // two row tiles share every weight tile (each loads half, multicast)
-        g.sched = 1;
-      }
-      g.stages = 2;
-      g.stages_b = gemm_halo_b_stages(g);
-      if (g.stages_b < 2) { set_error("layer " + w->name + ": halo pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
-    }
-    // (the 80 / 96-wide heads at three pieces fit one operand stage only: the producer then refills behind each k-block)
-    if (g.stages < 1) { set_error("layer " + w->name + ": pipeline does not fit shared memory"); return DAD3D_ERR_INVALID; }
-    for (int p = 0; p < enc->P; ++p) {
-      // stem: row x of the A operand is the 64-element window that starts at padded s2d pixel x (dim 1 advances by one
-      // 16-channel pixel = 32 bytes while the window is 128 bytes long: consecutive rows overlap)
-      const uint64_t dims[4] = {static_cast<uint64_t>(s.stem ? kBlockK : ti.C), static_cast<uint64_t>(s.stem ? Wo : ti.W),
-                                static_cast<uint64_t>(ti.H), static_cast<uint64_t>(ti.N)};
-      const uint64_t strides[3] = {static_cast<uint64_t>(ti.C) * 2, static_cast<uint64_t>(ti.W) * ti.C * 2,
-                                   static_cast<uint64_t>(ti.H) * ti.W * ti.C * 2};
-      const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(halo ? kHaloPW : g.tw * s.stride),
-                               static_cast<uint32_t>(halo ? kHaloPH : g.th * s.stride), static_cast<uint32_t>(g.tn)};
-      const uint32_t es[4] = {1, static_cast<uint32_t>(s.stride), static_cast<uint32_t>(s.stride), 1};
-      const uint16_t* basep = reinterpret_cast<const uint16_t*>(ti.ptr) + static_cast<size_t>(p) * ti.plane_elems();
-      if (!make_tmap_16bit(&s.maps.a[p], basep, 4, dims, strides, box, es)) return DAD3D_ERR_CUDA;
-      s.maps.b[p] = (block_n != w->block_n || g.cl_m == 2) ? w->map_b64[p] : w->map_b[p];
-    }
-    if (res_in_k || src2) {
-      const TensorInfo& tr = plan->tensors[s.res];
-      const int rs = src2 ? s.res_stride : 1;
-      for (int p = 0; p < enc->P; ++p) {
-        const uint64_t dims[4] = {static_cast<uint64_t>(tr.C), static_cast<uint64_t>(tr.W), static_cast<uint64_t>(tr.H),
-                                  static_cast<uint64_t>(tr.N)};
-        const uint64_t strides[3] = {static_cast<uint64_t>(tr.C) * 2, static_cast<uint64_t>(tr.W) * tr.C * 2,
-                                     static_cast<uint64_t>(tr.H) * tr.W * tr.C * 2};
-        const uint32_t box[4] = {kBlockK, static_cast<uint32_t>(g.tw * rs), static_cast<uint32_t>(g.th * rs),
-                                 static_cast<uint32_t>(g.tn)};
-        const uint32_t es[4] = {1, static_cast<uint32_t>(rs), static_cast<uint32_t>(rs), 1};
-        const uint16_t* basep = reinterpret_cast<const uint16_t*>(tr.ptr) + static_cast<size_t>(p) * tr.plane_elems();
-        if (!make_tmap_16bit(&s.maps.r[p], basep, 4, dims, strides, box, es)) return DAD3D_ERR_CUDA;
-      }
-    }
-    EpiConv::Params& ep = s.epi;
-    std::memset(&ep, 0, sizeof(ep));
-    ep.bias = w->d_bias;
-    ep.scale = w->d_scale;
-    ep.relu = s.relu;
-    ep.res_mode = (res_in_k || src2) ? 0 : s.res_mode;
-    ep.res = view(s.res);
-    ep.up2 = s.up2;
-    ep.parity = s.parity;
-    if (s.res >= 0 && !src2 && plan->tensors[s.res].C != w->cout_pad) {
-      set_error("layer " + w->name + ": residual channel mismatch");
-      return DAD3D_ERR_INVALID;
-    }
-    if (s.out >= 0) {
-      const TensorInfo& to = plan->tensors[s.out];
-      ep.out = reinterpret_cast<uint16_t*>(to.ptr);
-      ep.out_plane = to.plane_elems();
-      ep.out_planes = to.planes;
-      ep.ld_out = to.C;
-      if (block_n != 64 && block_n != 128) {
-        set_error("layer " + w->name + ": piece outputs need block_n 64 or 128");
-        return DAD3D_ERR_INVALID;
-      }
-      // per-warp store box: 16 consecutive tile rows = (bw x bh x bn) output pixels x 32 channels (SWIZZLE_64B rows)
-      const int nc = 32;
-      const int bw = std::min(g.tw, 16);
-      const int bh = std::min(g.th, 16 / bw);
-      const int bn = 16 / (bw * bh);
-      for (int p = 0; p < to.planes; ++p) {
-        uint16_t* basep = reinterpret_cast<uint16_t*>(to.ptr) + static_cast<size_t>(p) * to.plane_elems();
-        if (s.up2 || s.parity) {
-          // [N, 2Ho, 2Wo, C] seen as (C, b, j, a, n*Ho + i): pixel (2i + a, 2j + b); a box with b = a = 1 addresses the
-          // sub-grid of one parity, so the same staging tile is stored four times
-          const uint64_t C2 = static_cast<uint64_t>(to.C) * 2;
-          const uint64_t dims[5] = {static_cast<uint64_t>(to.C), 2, static_cast<uint64_t>(Wo), 2,
-                                    static_cast<uint64_t>(to.N) * Ho};
-          const uint64_t strides[4] = {C2, 2 * C2, static_cast<uint64_t>(to.W) * C2, 2 * static_cast<uint64_t>(to.W) * C2};
-          const uint32_t box[5] = {static_cast<uint32_t>(nc), 1, static_cast<uint32_t>(bw), 1, static_cast<uint32_t>(bh * bn)};
-          if (!make_tmap_16bit(&s.maps.c[p], basep, 5, dims, strides, box, nullptr, nc * 2)) return DAD3D_ERR_CUDA;
-          continue;
-        }
-        const uint64_t dims[4] = {static_cast<uint64_t>(to.C), static_cast<uint64_t>(to.W), static_cast<uint64_t>(to.H),
-                                  static_cast<uint64_t>(to.N)};
-        const uint64_t strides[3] = {static_cast<uint64_t>(to.C) * 2, static_cast<uint64_t>(to.W) * to.C * 2,
-                                     static_cast<uint64_t>(to.H) * to.W * to.C * 2};
-        const uint32_t box[4] = {static_cast<uint32_t>(nc), static_cast<uint32_t>(bw), static_cast<uint32_t>(bh),
-                                 static_cast<uint32_t>(bn)};
-        if (!make_tmap_16bit(&s.maps.c[p], basep, 4, dims, strides, box, nullptr, nc * 2)) return DAD3D_ERR_CUDA;
-      }
-    }
-    if (s.out_f32 >= 0) {
-      const TensorInfo& to = plan->tensors[s.out_f32];
-      ep.out_f32 = reinterpret_cast<float*>(to.ptr);
-      ep.ld_f32 = to.C;
-    }
+    if ((rc = conv_geometry(enc, *plan, s, &s.geom)) != DAD3D_OK) return rc;
+    if ((rc = conv_maps(enc, *plan, s)) != DAD3D_OK) return rc;
+    conv_epilogue(enc, *plan, s);
   }
   enc->plan = std::move(plan);
   return DAD3D_OK;
@@ -675,8 +686,8 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
     DAD3D_CUDA_OK(cudaEventRecord(ev->first, stream));
   }
   const int rc = enc->fp16
-                     ? gemm_launch<EpiConvH>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->use_pdl, stream)
-                     : gemm_launch<EpiConv>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->use_pdl, stream);
+                     ? gemm_launch<EpiConvH>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->sw.pdl, stream)
+                     : gemm_launch<EpiConv>(s.maps, s.geom, s.epi, enc->num_sms, &enc->gemm_cache, enc->sw.pdl, stream);
   if (rc != DAD3D_OK) return rc;
   if (ev) DAD3D_CUDA_OK(cudaEventRecord(ev->second, stream));
   return DAD3D_OK;
@@ -688,10 +699,7 @@ int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* pa
   const Plan& plan = *enc->plan;
   const int B = plan.B;
   auto T = [&](int id) -> const TensorInfo& { return plan.tensors[id]; };
-  auto view = [&](int id) {
-    const TensorInfo& t = T(id);
-    return ActView{reinterpret_cast<const uint16_t*>(t.ptr), t.plane_elems(), t.planes, t.C, enc->fp16};
-  };
+  auto view = [&](int id) { return T(id).view(enc->fp16); };
   switch (s.kind) {
     case kStemConv: {
       const TensorInfo& to = T(s.out_f32);
@@ -700,7 +708,7 @@ int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* pa
         DAD3D_CUDA_OK(cudaFuncSetAttribute(stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStemSmemBytes));
         enc->stem_configured = true;
       }
-      stem_conv_kernel<<<grid, 256, kStemSmemBytes, stream>>>(images_d, enc->d_stem_w, enc->d_stem_b, kImg, kImg,
+      stem_conv_kernel<<<grid, 256, kStemSmemBytes, stream>>>(images_d, enc->d_stem_w.get(), enc->d_stem_b.get(), kImg, kImg,
                                                  reinterpret_cast<float*>(to.ptr));
       count_launch();
       break;
@@ -786,6 +794,110 @@ int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* pa
   return DAD3D_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- weights
+// the SIMT stem's filter on the device: [(c * 7 + r) * 7 + s][64] from [64][7][7][3], and its bias
+int upload_stem(dad3d_encoder* enc, const dad3d_conv_weights& L) {
+  std::vector<float> w(147 * 64);
+  for (int o = 0; o < 64; ++o)
+    for (int r = 0; r < 7; ++r)
+      for (int s = 0; s < 7; ++s)
+        for (int c = 0; c < 3; ++c)
+          w[((c * 7 + r) * 7 + s) * 64 + o] = L.weight_h[((static_cast<size_t>(o) * 7 + r) * 7 + s) * 3 + c];
+  if (!upload(&enc->d_stem_w, w.data(), w.size()) || !upload(&enc->d_stem_b, L.bias_h, 64)) {
+    set_error("stem upload failed");
+    return DAD3D_ERR_CUDA;
+  }
+  return DAD3D_OK;
+}
+
+// the stem's 7x7/2 filter [64][7][7][3] re-expressed as 4x4/1 over the 2x2 space-to-depth image, [64][4][64]: K index =
+// r * 64 + dx * 16 + (py * 2 + px) * 3 + ch for block row / column offsets r, dx in 0..3 (s2d block oy - 2 + r,
+// ox - 2 + dx); the original tap is ky = 2 r + py - 1, kx = 2 dx + px - 1 (zero outside 0..6)
+std::vector<float> stem_as_s2d(const float* w7) {
+  std::vector<float> w4(static_cast<size_t>(64) * 4 * 64, 0.f);
+  for (int o = 0; o < 64; ++o)
+    for (int r = 0; r < 4; ++r)
+      for (int dx = 0; dx < 4; ++dx)
+        for (int py = 0; py < 2; ++py)
+          for (int px = 0; px < 2; ++px) {
+            const int ky = 2 * r + py - 1, kx = 2 * dx + px - 1;
+            if (ky < 0 || ky > 6 || kx < 0 || kx > 6) continue;
+            for (int c = 0; c < 3; ++c)
+              w4[(static_cast<size_t>(o) * 4 + r) * 64 + dx * 16 + (py * 2 + px) * 3 + c] =
+                  w7[((static_cast<size_t>(o) * 7 + ky) * 7 + kx) * 3 + c];
+          }
+  return w4;
+}
+
+// one layer as a tile-engine operand: its shape and padding, the weights as P bf16 / fp16 piece planes
+// [P][cout_pad][ktot] (identity columns included) with bias and scales on the device, and its B-operand tensor maps
+int pack_conv(const std::string& name, const dad3d_conv_weights& L, int pieces, int fp16, ConvW* cw) {
+  cw->name = name;
+  cw->cout = L.cout; cw->cin = L.cin; cw->R = L.R; cw->S = L.S;
+  cw->block_n = pick_block_n(L.cout);
+  cw->cout_pad = ceil_div(L.cout, cw->block_n) * cw->block_n;
+  cw->cin_pad = ceil_div(L.cin, kBlockK) * kBlockK;
+  // the last 1x1 of a ResUnit ("...c3") gets identity columns appended to its K axis: [W | I] * [a ; residual]
+  // (the first unit's c3 carries the projection-shortcut weights in its K axis instead and needs no identity)
+  cw->has_identity = name.size() > 4 && L.R == 1 && L.S == 1 &&
+                     ((name.compare(name.size() - 2, 2, "c3") == 0 && name.compare(name.size() - 4, 4, "u1c3") != 0) ||
+                      name.compare(name.size() - 2, 2, "td") == 0);      // BiFPN top-down nodes add the up-sampled branch
+  const size_t ktot_main = static_cast<size_t>(L.R) * L.S * cw->cin_pad;
+  const size_t ktot = ktot_main + (cw->has_identity ? cw->cout_pad : 0);
+  const size_t plane = static_cast<size_t>(cw->cout_pad) * ktot;
+  std::vector<uint16_t> packed(plane * pieces, 0);
+  // fp16 pieces: row o is stored as w * 2^s_o with max |w * 2^s_o| <= 2^15 (s_o <= 15 so that the identity entry 2^s_o
+  // stays representable); the epilogue multiplies the accumulator by 2^-s_o (exact).  bf16 pieces: s_o = 0.
+  std::vector<float> scale(cw->cout_pad, 1.f), up(cw->cout_pad, 1.f);
+  if (fp16)
+    for (int o = 0; o < L.cout; ++o) {
+      float amax = 0.f;
+      const float* row = L.weight_h + static_cast<size_t>(o) * L.R * L.S * L.cin;
+      for (size_t i = 0; i < static_cast<size_t>(L.R) * L.S * L.cin; ++i) amax = std::max(amax, std::fabs(row[i]));
+      int e = 0;
+      if (amax > 0.f && std::isfinite(amax)) {
+        std::frexp(amax, &e);                       // amax = m * 2^e, m in [0.5, 1)  ->  amax * 2^(15 - e) in [2^14, 2^15)
+        e = std::min(15, 15 - e);
+        e = std::max(e, -100);
+      }
+      up[o] = std::ldexp(1.f, e);
+      scale[o] = std::ldexp(1.f, -e);
+    }
+  if (cw->has_identity)
+    for (int o = 0; o < cw->cout_pad; ++o)
+      packed[static_cast<size_t>(o) * ktot + ktot_main + o] = fp16 ? host_f16(up[o]) : static_cast<uint16_t>(0x3F80);   // piece 0
+  for (int o = 0; o < L.cout; ++o)
+    for (int t = 0; t < L.R * L.S; ++t)
+      for (int c = 0; c < L.cin; ++c) {
+        float r = L.weight_h[(static_cast<size_t>(o) * L.R * L.S + t) * L.cin + c] * up[o];
+        const size_t idx = static_cast<size_t>(o) * ktot + static_cast<size_t>(t) * cw->cin_pad + c;
+        for (int p = 0; p < pieces; ++p) {
+          const uint16_t h = fp16 ? host_f16(r) : host_bf16(r);
+          packed[p * plane + idx] = h;
+          r -= fp16 ? host_f16_to_f32(h) : host_bf16_to_f32(h);
+        }
+      }
+  std::vector<float> bias(cw->cout_pad, 0.f);
+  for (int o = 0; o < L.cout; ++o) bias[o] = L.bias_h[o];
+  if (!upload(&cw->d_w, packed.data(), packed.size()) || !upload(&cw->d_bias, bias.data(), bias.size()) ||
+      !upload(&cw->d_scale, scale.data(), scale.size())) {
+    set_error("weight upload failed for " + name);
+    return DAD3D_ERR_CUDA;
+  }
+  // B maps: box 64 x block_n, and 64 x 64 for the 128-wide layers
+  const uint64_t dims[2] = {static_cast<uint64_t>(ktot), static_cast<uint64_t>(cw->cout_pad)};
+  const uint64_t strides[1] = {static_cast<uint64_t>(ktot) * 2};
+  const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(cw->block_n)};
+  const uint32_t box64[2] = {kBlockK, 64};
+  cw->has_b64 = cw->block_n == 128;
+  for (int p = 0; p < pieces; ++p) {
+    if (!make_tmap_16bit(&cw->map_b[p], cw->d_w.get() + p * plane, 2, dims, strides, box, nullptr)) return DAD3D_ERR_CUDA;
+    if (cw->has_b64 && !make_tmap_16bit(&cw->map_b64[p], cw->d_w.get() + p * plane, 2, dims, strides, box64, nullptr))
+      return DAD3D_ERR_CUDA;
+  }
+  return DAD3D_OK;
+}
+
 }  // namespace
 
 // =================================================================================================== C ABI
@@ -810,166 +922,49 @@ int dad3d_encoder_create(dad3d_encoder** out, const dad3d_conv_weights* layers, 
   enc->P = pieces;
   enc->fp16 = operand_format == DAD3D_OPERAND_FP16 ? 1 : 0;
   std::memcpy(enc->bifpn_w, bifpn_fusion_w_h, sizeof(enc->bifpn_w));
-  {
-    const char* e = std::getenv("DAD3D_PDL");
-    enc->use_pdl = (e && e[0] == '1');
-    const char* e4 = std::getenv("DAD3D_HALO");
-    enc->use_halo = !(e4 && e4[0] == '0');
-    const char* e5 = std::getenv("DAD3D_HALO_CLUSTER");
-    enc->halo_cluster = (e5 && e5[0] == '2') ? 2 : 1;
-    const char* e6 = std::getenv("DAD3D_TD_PARITY");
-    enc->td_parity = (e6 && e6[0] == '1');
-    const char* e9 = std::getenv("DAD3D_HEAT_SPARSE");
-    enc->heat_sparse = !(e9 && std::atoi(e9) == 0);
-    const char* e2 = std::getenv("DAD3D_STEM_SIMT");
-    enc->stem_simt = (e2 && e2[0] == '1');
-  }
+  enc->sw = read_switches();
 
-  auto fail = [&](int code) { dad3d_encoder_destroy(enc.release()); return code; };
-  std::vector<float> stem_w4;                      // the stem's 7x7/2 filter re-expressed as 4x4/1 over the 2x2 space-to-depth image
+  std::vector<float> stem_w4;
   for (int li = 0; li < n_layers; ++li) {
     dad3d_conv_weights L = layers[li];
     if (!L.name || !L.weight_h || !L.bias_h || L.cout <= 0 || L.cin <= 0 || L.R <= 0 || L.S <= 0) {
       set_error("invalid layer record " + std::to_string(li));
-      return fail(DAD3D_ERR_INVALID);
+      return DAD3D_ERR_INVALID;
     }
     const std::string name(L.name);
     if (name == "stem") {
-      if (L.cout != 64 || L.cin != 3 || L.R != 7 || L.S != 7) { set_error("stem must be 7x7 3->64"); return fail(DAD3D_ERR_INVALID); }
-      std::vector<float> w(147 * 64);
-      for (int o = 0; o < 64; ++o)
-        for (int r = 0; r < 7; ++r)
-          for (int s = 0; s < 7; ++s)
-            for (int c = 0; c < 3; ++c)       // input [cout][R][S][cin] -> [(c*7+r)*7+s][cout]
-              w[((c * 7 + r) * 7 + s) * 64 + o] = L.weight_h[((static_cast<size_t>(o) * 7 + r) * 7 + s) * 3 + c];
-      if (cudaMalloc(&enc->d_stem_w, w.size() * 4) != cudaSuccess || cudaMalloc(&enc->d_stem_b, 64 * 4) != cudaSuccess ||
-          cudaMemcpy(enc->d_stem_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
-          cudaMemcpy(enc->d_stem_b, L.bias_h, 64 * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
-        set_error("stem upload failed");
-        return fail(DAD3D_ERR_CUDA);
-      }
-      // tensor-core stem: K index = r * 64 + dx * 16 + (py * 2 + px) * 3 + ch for block row/column offsets r, dx in 0..3
-      // (s2d block oy - 2 + r, ox - 2 + dx); the original tap is ky = 2 r + py - 1, kx = 2 dx + px - 1 (zero outside 0..6)
-      stem_w4.assign(static_cast<size_t>(64) * 4 * 64, 0.f);
-      for (int o = 0; o < 64; ++o)
-        for (int r = 0; r < 4; ++r)
-          for (int dx = 0; dx < 4; ++dx)
-            for (int py = 0; py < 2; ++py)
-              for (int px = 0; px < 2; ++px) {
-                const int ky = 2 * r + py - 1, kx = 2 * dx + px - 1;
-                if (ky < 0 || ky > 6 || kx < 0 || kx > 6) continue;
-                for (int c = 0; c < 3; ++c)
-                  stem_w4[(static_cast<size_t>(o) * 4 + r) * 64 + dx * 16 + (py * 2 + px) * 3 + c] =
-                      L.weight_h[((static_cast<size_t>(o) * 7 + ky) * 7 + kx) * 3 + c];
-              }
+      if (L.cout != 64 || L.cin != 3 || L.R != 7 || L.S != 7) { set_error("stem must be 7x7 3->64"); return DAD3D_ERR_INVALID; }
+      const int rc = upload_stem(enc.get(), L);
+      if (rc != DAD3D_OK) return rc;
+      stem_w4 = stem_as_s2d(L.weight_h);            // the tensor-core stem is packed as a 4x4 conv over 64 channels
       L.weight_h = stem_w4.data();
-      L.cin = 64; L.R = 4; L.S = 1;                 // falls through to the generic packing below
+      L.cin = 64; L.R = 4; L.S = 1;
     }
     ConvW cw;
-    cw.name = name;
-    cw.cout = L.cout; cw.cin = L.cin; cw.R = L.R; cw.S = L.S;
-    cw.block_n = pick_block_n(L.cout);
-    cw.cout_pad = ceil_div(L.cout, cw.block_n) * cw.block_n;
-    cw.cin_pad = ceil_div(L.cin, kBlockK) * kBlockK;
-    // the last 1x1 of a ResUnit ("...c3") gets identity columns appended to its K axis: [W | I] * [a ; residual]
-    // (the first unit's c3 carries the projection-shortcut weights in its K axis instead and needs no identity)
-    cw.has_identity = name.size() > 4 && L.R == 1 && L.S == 1 &&
-                      ((name.compare(name.size() - 2, 2, "c3") == 0 && name.compare(name.size() - 4, 4, "u1c3") != 0) ||
-                       name.compare(name.size() - 2, 2, "td") == 0);      // BiFPN top-down nodes add the up-sampled branch
-    const size_t ktot_main = static_cast<size_t>(L.R) * L.S * cw.cin_pad;
-    const size_t ktot = ktot_main + (cw.has_identity ? cw.cout_pad : 0);
-    const size_t plane = static_cast<size_t>(cw.cout_pad) * ktot;
-    std::vector<uint16_t> packed(plane * pieces, 0);
-    // fp16 pieces: row o is stored as w * 2^s_o with max |w * 2^s_o| <= 2^15 (s_o <= 15 so that the identity entry 2^s_o
-    // stays representable); the epilogue multiplies the accumulator by 2^-s_o (exact).  bf16 pieces: s_o = 0.
-    std::vector<float> scale(cw.cout_pad, 1.f), up(cw.cout_pad, 1.f);
-    if (enc->fp16)
-      for (int o = 0; o < L.cout; ++o) {
-        float amax = 0.f;
-        const float* row = L.weight_h + static_cast<size_t>(o) * L.R * L.S * L.cin;
-        for (size_t i = 0; i < static_cast<size_t>(L.R) * L.S * L.cin; ++i) amax = std::max(amax, std::fabs(row[i]));
-        int e = 0;
-        if (amax > 0.f && std::isfinite(amax)) {
-          std::frexp(amax, &e);                       // amax = m * 2^e, m in [0.5, 1)  ->  amax * 2^(15 - e) in [2^14, 2^15)
-          e = std::min(15, 15 - e);
-          e = std::max(e, -100);
-        }
-        up[o] = std::ldexp(1.f, e);
-        scale[o] = std::ldexp(1.f, -e);
-      }
-    if (cw.has_identity)
-      for (int o = 0; o < cw.cout_pad; ++o)
-        packed[static_cast<size_t>(o) * ktot + ktot_main + o] = enc->fp16 ? host_f16(up[o]) : static_cast<uint16_t>(0x3F80);   // piece 0
-    for (int o = 0; o < L.cout; ++o)
-      for (int t = 0; t < L.R * L.S; ++t)
-        for (int c = 0; c < L.cin; ++c) {
-          float r = L.weight_h[(static_cast<size_t>(o) * L.R * L.S + t) * L.cin + c] * up[o];
-          const size_t idx = static_cast<size_t>(o) * ktot + static_cast<size_t>(t) * cw.cin_pad + c;
-          for (int p = 0; p < pieces; ++p) {
-            const uint16_t h = enc->fp16 ? host_f16(r) : host_bf16(r);
-            packed[p * plane + idx] = h;
-            r -= enc->fp16 ? host_f16_to_f32(h) : host_bf16_to_f32(h);
-          }
-        }
-    std::vector<float> bias(cw.cout_pad, 0.f);
-    for (int o = 0; o < L.cout; ++o) bias[o] = L.bias_h[o];
-    if (cudaMalloc(&cw.d_w, packed.size() * 2) != cudaSuccess || cudaMalloc(&cw.d_bias, bias.size() * 4) != cudaSuccess ||
-        cudaMalloc(&cw.d_scale, scale.size() * 4) != cudaSuccess ||
-        cudaMemcpy(cw.d_scale, scale.data(), scale.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(cw.d_w, packed.data(), packed.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(cw.d_bias, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
-      set_error("weight upload failed for " + name);
-      cudaFree(cw.d_w); cudaFree(cw.d_bias); cudaFree(cw.d_scale);
-      return fail(DAD3D_ERR_CUDA);
-    }
-    for (int p = 0; p < pieces; ++p) {
-      const uint64_t dims[2] = {static_cast<uint64_t>(ktot), static_cast<uint64_t>(cw.cout_pad)};
-      const uint64_t strides[1] = {static_cast<uint64_t>(ktot) * 2};
-      const uint32_t box[2] = {kBlockK, static_cast<uint32_t>(cw.block_n)};
-      if (!make_tmap_16bit(&cw.map_b[p], cw.d_w + p * plane, 2, dims, strides, box, nullptr)) {
-        cudaFree(cw.d_w); cudaFree(cw.d_bias); cudaFree(cw.d_scale);
-        return fail(DAD3D_ERR_CUDA);
-      }
-      if (cw.block_n == 128) {
-        const uint32_t box64[2] = {kBlockK, 64};
-        if (!make_tmap_16bit(&cw.map_b64[p], cw.d_w + p * plane, 2, dims, strides, box64, nullptr)) {
-          cudaFree(cw.d_w); cudaFree(cw.d_bias); cudaFree(cw.d_scale);
-          return fail(DAD3D_ERR_CUDA);
-        }
-        cw.has_b64 = true;
-      }
-    }
-    enc->convs[name] = cw;
+    const int rc = pack_conv(name, L, pieces, enc->fp16, &cw);
+    if (rc != DAD3D_OK) return rc;
+    enc->convs[name] = std::move(cw);
   }
   // every layer the graph needs must be present
-  {
-    std::vector<std::string> need = {"lat4", "lat5", "lat6", "lat7", "heat", "fusion", "mlp1", "mlp2"};
-    for (int si = 0; si < 4; ++si)
-      for (int ui = 0; ui < kStageUnits[si]; ++ui) {
-        const std::string p = "s" + std::to_string(si + 1) + "u" + std::to_string(ui + 1);
-        need.push_back(p + "c1"); need.push_back(p + "c2"); need.push_back(p + "c3");
-      }
-    for (int li = 0; li < 2; ++li)
-      for (const char* n : {"p6td", "p5td", "p4td", "p3td", "p6td_u", "p5td_u", "p4td_u", "p3td_u", "p4out", "p5out",
-                            "p6out", "p7out"})
-        need.push_back("b" + std::to_string(li) + "_" + n);
-    for (auto& n : need)
-      if (!enc->convs.count(n)) { set_error("missing layer weights: " + n); return fail(DAD3D_ERR_INVALID); }
-    if (!enc->d_stem_w) { set_error("missing layer weights: stem"); return fail(DAD3D_ERR_INVALID); }
-  }
+  std::vector<std::string> need = {"lat4", "lat5", "lat6", "lat7", "heat", "fusion", "mlp1", "mlp2"};
+  for (int si = 0; si < 4; ++si)
+    for (int ui = 0; ui < kStageUnits[si]; ++ui) {
+      const std::string p = "s" + std::to_string(si + 1) + "u" + std::to_string(ui + 1);
+      need.push_back(p + "c1"); need.push_back(p + "c2"); need.push_back(p + "c3");
+    }
+  for (int li = 0; li < 2; ++li)
+    for (const char* n : {"p6td", "p5td", "p4td", "p3td", "p6td_u", "p5td_u", "p4td_u", "p3td_u", "p4out", "p5out",
+                          "p6out", "p7out"})
+      need.push_back("b" + std::to_string(li) + "_" + n);
+  for (auto& n : need)
+    if (!enc->convs.count(n)) { set_error("missing layer weights: " + n); return DAD3D_ERR_INVALID; }
+  if (!enc->d_stem_w) { set_error("missing layer weights: stem"); return DAD3D_ERR_INVALID; }
   *out = enc.release();
   return DAD3D_OK;
 }
 
 void dad3d_encoder_destroy(dad3d_encoder* enc) {
   if (!enc) return;
-  for (auto& kv : enc->convs) {
-    cudaFree(kv.second.d_w);
-    cudaFree(kv.second.d_bias);
-    cudaFree(kv.second.d_scale);
-  }
-  cudaFree(enc->d_stem_w);
-  cudaFree(enc->d_stem_b);
   for (auto& ev : enc->prof_events) {
     cudaEventDestroy(ev.first);
     cudaEventDestroy(ev.second);
@@ -1093,8 +1088,8 @@ int dad3d_encoder_read_activation(dad3d_encoder* enc, const char* name, float* o
     if (t.f32) {
       DAD3D_CUDA_OK(cudaMemcpyAsync(out_d, t.ptr, n * 4, cudaMemcpyDeviceToDevice, stream));
     } else {
-      ActView v{reinterpret_cast<const uint16_t*>(t.ptr), t.plane_elems(), t.planes, t.C, enc->fp16};
-      pieces_to_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(v, static_cast<long long>(n), out_d);
+      pieces_to_f32_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(t.view(enc->fp16),
+                                                                                      static_cast<long long>(n), out_d);
       count_launch();
       DAD3D_CUDA_OK(cudaGetLastError());
     }
@@ -1142,8 +1137,8 @@ int dad3d_encoder_describe_plan(dad3d_encoder* enc, char* buf, size_t cap) {
       num("cout", s.w->cout); num("cin", s.w->cin); num("has_identity", s.w->has_identity ? 1 : 0);
       cudaLaunchConfig_t cfg;
       cudaLaunchAttribute attr[2];
-      const int rc = enc->fp16 ? gemm_launch_config<EpiConvH>(g, enc->num_sms, &enc->gemm_cache, enc->use_pdl, &cfg, attr)
-                               : gemm_launch_config<EpiConv>(g, enc->num_sms, &enc->gemm_cache, enc->use_pdl, &cfg, attr);
+      const int rc = enc->fp16 ? gemm_launch_config<EpiConvH>(g, enc->num_sms, &enc->gemm_cache, enc->sw.pdl, &cfg, attr)
+                               : gemm_launch_config<EpiConv>(g, enc->num_sms, &enc->gemm_cache, enc->sw.pdl, &cfg, attr);
       if (rc != DAD3D_OK) return rc;
       const int grid = static_cast<int>(cfg.gridDim.x);
       int tmin = 1 << 30, tmax = 0;

@@ -1,5 +1,6 @@
-"""Ping-pong tile engine on the CPU: a restatement of make_plan's tile choice for every conv launch of the encoder, and a
-model of the pipeline protocol of a ping-pong launch (tile_gemm.cuh, gemm_consumer_pingpong).
+"""Ping-pong tile engine on the CPU: a restatement of the tile choice for every conv launch of the encoder (geometry()
+follows conv_geometry in csrc/encoder.cu decision by decision, in the same order), and a model of the pipeline protocol
+of a ping-pong launch (tile_gemm.cuh, gemm_consumer_pingpong).
 
 The protocol model runs the TMA producer, the two consumer warpgroups, the shared-memory ring (full / empty mbarriers
 with phase parity) and the order barrier (turn_bar) as interleaved agents under a seeded random schedule.  TMA loads
@@ -10,7 +11,7 @@ import dataclasses
 import random
 from typing import Dict, List, Optional
 
-# ------------------------------------------------------------------------------------------- make_plan, restated
+# ------------------------------------------------------------------------------------------- conv_geometry, restated
 NUM_SMS = 132
 SMEM_LIMIT = 227 * 1024
 TILE_A = 128 * 64 * 2
@@ -126,7 +127,8 @@ def network(B: int, td_parity: bool = False, heat_sparse: bool = True) -> List[L
 
 
 def geometry(ln: Launch, P: int, use_halo: bool = True) -> Dict[str, int]:
-    """The GemmGeom fields (and launch grid) make_plan derives for one launch, as describe_plan names them."""
+    """The GemmGeom fields (and launch grid) conv_geometry derives for one launch, as describe_plan names them; in the
+    order of conv_geometry, so that the two read side by side."""
     bn_w = pick_block_n(ln.cout)
     cout_pad = _ceil(ln.cout, bn_w) * bn_w
     has_b64 = bn_w == 128

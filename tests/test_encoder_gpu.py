@@ -183,3 +183,51 @@ def test_encoder_reference_fixture(sd, cuda_device):
         assert _rel(out[OUTPUT_2D_LANDMARKS], torch.from_numpy(z["landmarks_f64"])) < 3e-5, mode
         assert _rel(out[OUTPUT_LANDMARKS_HEATMAP].sum(dim=(2, 3)), torch.from_numpy(z["heatmap_sum_f64"])) < 3e-5, mode
         assert _rel(out[OUTPUT_LANDMARKS_HEATMAP][:, :, :4, :4], torch.from_numpy(z["heatmap_corner_f64"])) < 1e-4, mode
+
+
+def test_create_rejects_invalid_weights(sd, cuda_device):
+    """dad3d_encoder_create refuses malformed weights with DAD3D_ERR_INVALID (-1) and says why: a record with a null or
+    non-positive field, a stem that is not 7x7 3->64, a layer the graph needs but no record carries, pieces or operand
+    format out of range."""
+    import ctypes as C
+    import numpy as np
+    from dad_3dheads_b200 import _lib
+    from dad_3dheads_b200.encoder import Dad3dEncoder, _ConvWeights, fold_state_dict
+    layers, fw = fold_state_dict(sd)
+    layers = [(n, np.ascontiguousarray(w, dtype=np.float32), np.ascontiguousarray(b, dtype=np.float32))
+              for n, w, b in layers]
+
+    def rejected(ls):
+        with pytest.raises(_lib.Dad3dError) as e:
+            Dad3dEncoder.from_folded(ls, fw, cuda_device, precision="fp16x2")
+        assert "(rc=-1)" in str(e.value), str(e.value)
+        return str(e.value)
+
+    stem = next(i for i, (n, _, _) in enumerate(layers) if n == "stem")
+    assert "missing layer weights: lat4" in rejected([l for l in layers if l[0] != "lat4"])
+    assert "missing layer weights: b1_p3td_u" in rejected([l for l in layers if l[0] != "b1_p3td_u"])
+    assert "missing layer weights: stem" in rejected([l for l in layers if l[0] != "stem"])
+    bad_stem = list(layers)
+    bad_stem[stem] = ("stem", np.zeros((64, 5, 5, 3), np.float32), layers[stem][2])
+    assert "stem must be 7x7 3->64" in rejected(bad_stem)
+    bad_stem[stem] = ("stem", np.zeros((64, 7, 7, 4), np.float32), layers[stem][2])
+    assert "stem must be 7x7 3->64" in rejected(bad_stem)
+    empty = list(layers)
+    empty.insert(3, ("lat4", np.zeros((0, 1, 1, 512), np.float32), np.zeros(0, np.float32)))
+    assert "invalid layer record 3" in rejected(empty)
+
+    lib = _lib.load()
+    name, w, b = layers[stem]
+    rec = (_ConvWeights * 1)()
+    rec[0].name, rec[0].weight_h, rec[0].bias_h = name.encode(), w.ctypes.data, b.ctypes.data
+    rec[0].cout, rec[0].R, rec[0].S, rec[0].cin = w.shape
+    fwc = np.ascontiguousarray(fw, dtype=np.float32)
+    for pieces, fmt, msg in [(0, 0, "pieces must be"), (4, 0, "pieces must be"), (3, 1, "operand_format must be"),
+                             (2, 2, "operand_format must be"), (1, -1, "operand_format must be")]:
+        h = C.c_void_p()
+        assert lib.dad3d_encoder_create(C.byref(h), rec, 1, fwc.ctypes.data, pieces, fmt, cuda_device.index) == -1
+        assert not h.value and msg in lib.dad3d_last_error().decode(), (pieces, fmt)
+    null = (_ConvWeights * 1)()
+    h = C.c_void_p()
+    assert lib.dad3d_encoder_create(C.byref(h), null, 1, fwc.ctypes.data, 1, 0, cuda_device.index) == -1
+    assert "invalid layer record 0" in lib.dad3d_last_error().decode()
