@@ -3,11 +3,9 @@ losses/*.py): index-set loading (model_training/utils.py:56-105), the logger fac
 (:108-117).  hydra / omegaconf / coloredlogs are not needed here (they only serve the training entry point)."""
 import logging
 import os
-from typing import Any, Dict, List, Tuple
+from typing import Any, Dict, List
 
-import numpy as np
-
-from dad_3dheads_b200.flame_assets import get_list_of_npy_files, load_indices_from_npy  # noqa: F401
+from dad_3dheads_b200.flame_assets import get_list_of_npy_files, indices_reweighing, load_indices_from_npy  # noqa: F401
 
 
 def create_logger(name: str, msg_format: str = "") -> logging.Logger:
@@ -35,13 +33,3 @@ def load_2d_indices(config: Dict[str, Any]) -> List[int]:
         else:
             raise ValueError(f"[{filename.split('.')[0].split('/')[-1]}] class of keypoints doesn't exist")
     return indices
-
-
-def indices_reweighing(weights_and_indices: Dict[str, Any]) -> Tuple[List, List]:
-    weights_dict = weights_and_indices["weights"]
-    weights, indices = [], []
-    for key, value in weights_and_indices["flame_indices"]["files"].items():
-        if key in weights_dict.keys():
-            indices.append(np.load(os.path.join(weights_and_indices["flame_indices"]["folder"], value)))
-            weights.append(weights_dict[key])
-    return weights, indices

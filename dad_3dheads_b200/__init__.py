@@ -6,5 +6,7 @@ compute classes without the built library, or calling them without a Hopper GPU,
 """
 from .flame import FLAME_CONSTS, FlameParams, FLAMELayer  # noqa: F401
 from .head_mesh import HeadMesh  # noqa: F401
+from .losses import IoULoss, LandmarksLossWVisibility, ReprojectionLoss, Vertices3DLoss  # noqa: F401
 
-__all__ = ["FLAME_CONSTS", "FlameParams", "FLAMELayer", "HeadMesh"]
+__all__ = ["FLAME_CONSTS", "FlameParams", "FLAMELayer", "HeadMesh", "IoULoss", "LandmarksLossWVisibility", "ReprojectionLoss",
+           "Vertices3DLoss"]

@@ -128,7 +128,26 @@ SIGNATURES = {
     "dad3d_encoder_write_activation": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dad3d_encoder_run_steps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p]),
+    "dad3d_iou_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_iou_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
+    "dad3d_landmarks_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_landmarks_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_vsub_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                    C.c_int32]),
+    "dad3d_vsub_destroy": (None, [C.c_void_p]),
+    "dad3d_vsub_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_vsub_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
+
+DAD3D_LOSS_L1 = 0
+DAD3D_LOSS_L2 = 1
+DAD3D_LOSS_SMOOTH_L1 = 2
+DAD3D_VSUB_RECORD_FLOATS = 32
 
 
 def load():

@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import os
 import pickle
-from typing import Dict, Optional
+from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
 
@@ -113,6 +113,18 @@ def get_list_of_npy_files(config: Dict) -> list:
         if stem in stems:
             stems.remove(stem)                            # first occurrence only, like list.remove in the reference
     return [os.path.join(folder, stem + ".npy") for stem in stems]
+
+
+def indices_reweighing(weights_and_indices: Dict[str, Any]) -> Tuple[List, List]:
+    """model_training/utils.py:108-117: the (weight, index array) pairs of the loss subsets, in the order of the
+    ``flame_indices.files`` mapping, for every file whose key has a weight."""
+    weights_dict = weights_and_indices["weights"]
+    weights, indices = [], []
+    for key, value in weights_and_indices["flame_indices"]["files"].items():
+        if key in weights_dict.keys():
+            indices.append(np.load(os.path.join(weights_and_indices["flame_indices"]["folder"], value)))
+            weights.append(weights_dict[key])
+    return weights, indices
 
 
 def load_static(path: Optional[str], default_npz: str) -> Dict[str, np.ndarray]:

@@ -449,6 +449,57 @@ DAD3D_API int dad3d_overlay_mesh(const float* vertices_d, int32_t R, int32_t nv,
                                  int32_t E, const dad3d_roi* rois_d, const uint8_t* color_h, int32_t* ws_d,
                                  uint8_t* frames_d, int32_t F, int32_t H, int32_t W, dad3d_stream stream);
 
+/* ---- training losses: the reference's train_loss.yaml objective and its gradients ---------------------------------
+ * Forward and backward are separate calls.  Reductions are per plane / per head partial sums, then one sum in a fixed
+ * order (no floating-point atomics): bit-reproducible, and one head's values never reach another head's gradient.  Every
+ * backward reads the incoming scalar loss gradient grad_out_d from device memory; nothing synchronises with the host, so a
+ * forward and backward can be captured in a CUDA graph.  loss_d is one fp32 scalar.  All tensors are contiguous fp32.
+ * criterion: the reference's l1 / l2 / smooth_l1 (nn.L1Loss, nn.MSELoss, nn.SmoothL1Loss with beta 1, mean reduction). */
+#define DAD3D_LOSS_L1 0
+#define DAD3D_LOSS_L2 1
+#define DAD3D_LOSS_SMOOTH_L1 2
+
+/*   dad3d_iou_forward / _backward  replace IoULoss (losses/keypoint_losses.py:5-31): x_d logits and t_d targets
+ *     [planes = B*C, hw = H*W].  Forward: s = sigmoid(x); stats_d [planes, 4] = (I = sum s t, T = sum t^2, S = sum s^2, iou =
+ *     (I + 1e-6) / (T + S - I + 1e-6)) and loss = 1 - mean iou (2 kernels).  Backward: grad_x_d = d loss / d x from stats_d
+ *     (1 kernel). */
+DAD3D_API int dad3d_iou_forward(const float* x_d, const float* t_d, int32_t planes, int32_t hw, float* stats_d, float* loss_d,
+                                dad3d_stream stream);
+DAD3D_API int dad3d_iou_backward(const float* x_d, const float* t_d, int32_t planes, int32_t hw, const float* stats_d,
+                                 const float* grad_out_d, float* grad_x_d, dad3d_stream stream);
+
+/*   dad3d_landmarks_forward / _backward  replace LandmarksLossWVisibility (losses/landmarks_loss_w_visibility.py:10-26):
+ *     criterion(p * p_presence, t * t_presence) with p_d, t_d [B,N,2] and the presences [B,N]; partial_d [B] per-head sums
+ *     (2 kernels).  Backward: grad_p_d [B,N,2] (the only input that receives a gradient; 1 kernel). */
+DAD3D_API int dad3d_landmarks_forward(const float* p_d, const float* p_presence_d, const float* t_d, const float* t_presence_d,
+                                      int32_t B, int32_t N, int32_t criterion, float* partial_d, float* loss_d,
+                                      dad3d_stream stream);
+DAD3D_API int dad3d_landmarks_backward(const float* p_d, const float* p_presence_d, const float* t_d,
+                                       const float* t_presence_d, int32_t B, int32_t N, int32_t criterion,
+                                       const float* grad_out_d, float* grad_p_d, dad3d_stream stream);
+
+/*   vertex-subset losses  replace the per-subset loops of Vertices3DLoss (losses/vertices_3d_loss.py:41-48, with
+ *     normalize_to_cube, model/utils.py:55-68, on both operands) and ReprojectionLoss (losses/reprojection_loss.py:33-46):
+ *     loss = sum_s w_s * mean_{B x |I_s| x K} criterion(f(v[:, I_s]) - f(t[:, I_s])), f = normalize_to_cube (normalize != 0)
+ *     or the identity, over the ordered index sets of indices_reweighing (model_training/utils.py:108-117).
+ *   dad3d_vsub_create  builds the set tables on `device`: indices_h [offsets_h[S]] holds the sets one after the other,
+ *     offsets_h [S + 1] (offsets_h[0] = 0, no empty set), weights_h [S], every index in [0, V).  Also builds the vertex ->
+ *     (set, position) lists the backward sums in a fixed order.
+ *   dad3d_vsub_forward  v_d, t_d [B,V,K] (K = 2 or 3) -> records_d [B, S, DAD3D_VSUB_RECORD_FLOATS] (per head and set: the
+ *     criterion sum and, when normalising, the reductions, the entries they selected -- the first extreme on ties, as torch's
+ *     min / max select -- and the sums the backward needs) and the loss (2 kernels).
+ *   dad3d_vsub_backward  grad_v_d [B,V,K] = d loss / d v, zero outside every set, from the forward's records (1 kernel). */
+typedef struct dad3d_vsub dad3d_vsub;
+#define DAD3D_VSUB_RECORD_FLOATS 32
+DAD3D_API int dad3d_vsub_create(dad3d_vsub** out, const int32_t* indices_h, const int32_t* offsets_h, const float* weights_h,
+                                int32_t S, int32_t V, int32_t device);
+DAD3D_API void dad3d_vsub_destroy(dad3d_vsub* h);
+DAD3D_API int dad3d_vsub_forward(const dad3d_vsub* h, const float* v_d, const float* t_d, int32_t B, int32_t K,
+                                 int32_t normalize, int32_t criterion, float* records_d, float* loss_d, dad3d_stream stream);
+DAD3D_API int dad3d_vsub_backward(const dad3d_vsub* h, const float* v_d, const float* t_d, int32_t B, int32_t K,
+                                  int32_t normalize, int32_t criterion, const float* records_d, const float* grad_out_d,
+                                  float* grad_v_d, dad3d_stream stream);
+
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
 
