@@ -142,6 +142,11 @@ SIGNATURES = {
                                      C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_vsub_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_training_targets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]),
+    "dad3d_heatmap_targets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                                        C.c_void_p, C.c_void_p]),
 }
 
 DAD3D_LOSS_L1 = 0

@@ -115,6 +115,19 @@ def get_list_of_npy_files(config: Dict) -> list:
     return [os.path.join(folder, stem + ".npy") for stem in stems]
 
 
+def load_2d_indices(config: Dict) -> Optional[List[int]]:
+    """model_training/utils.py:62-78: the 2D keypoint subset -- None for ``2d_subset_name == "multipie_keypoints"`` (the 68
+    barycentric landmarks), else the index lists of ``get_list_of_npy_files`` concatenated over the SORTED file names."""
+    if config["2d_subset_name"] == "multipie_keypoints":
+        return None
+    indices: List[int] = []
+    for filename in sorted(get_list_of_npy_files(config)):
+        if not os.path.exists(filename):
+            raise ValueError(f"[{filename.split('.')[0].split('/')[-1]}] class of keypoints doesn't exist")
+        indices += load_indices_from_npy(filename)
+    return indices
+
+
 def indices_reweighing(weights_and_indices: Dict[str, Any]) -> Tuple[List, List]:
     """model_training/utils.py:108-117: the (weight, index array) pairs of the loss subsets, in the order of the
     ``flame_indices.files`` mapping, for every file whose key has a weight."""

@@ -500,6 +500,33 @@ DAD3D_API int dad3d_vsub_backward(const dad3d_vsub* h, const float* v_d, const f
                                   int32_t normalize, int32_t criterion, const float* records_d, const float* grad_out_d,
                                   float* grad_v_d, dad3d_stream stream);
 
+/* ---- training targets: the reference's FlameDataset batch after the crop ----------------------------------------------
+ * The letter-boxed images come from dad3d_roi_setup (boxes (0, 0, w, h), zero extend, one frame per crop) and
+ * dad3d_preprocess_rois; these two calls make the rest.  Each launches one kernel, with no floating-point atomics and no
+ * host synchronisation.  Float arithmetic is in an explicit order of single roundings (tests/targets_model.py restates it).
+ *   dad3d_training_targets  replaces FlameDataset._load_mesh's world transform, _get_2d_landmarks_w_presence,
+ *     _project_vertices_onto_image and the keypoint path of _transform (model_training/data/flame_dataset.py:115-192), one
+ *     CTA per head.  vertices_d [B,V,3] model space, model_view_d and projection_d [B,4,4] row-major, origins_d [B,3] int32
+ *     (crop x, crop y in frame pixels, frame height), rois_d the records of the crops (w, h, scale, pre_left, pre_top).
+ *     Landmarks: lm_tri_d [C,3] vertex indices with lm_bary_d [C,3] barycentric weights (get_68_landmarks, data/utils.py:
+ *     190-206: dynamic zero-pose row then static, projected as [lm, 1]), or lm_index_d [C] (world_homo[indices], projected
+ *     with the computed w); exactly one of the two.  Outputs: keypoints_d [B,V,2] and landmarks_d [B,C,2] in network
+ *     pixels (fp32(fp32(x * fp32(scale)) + pad)), landmarks_norm_d = landmarks_d / img_size, presence_d [B,C] uint8
+ *     (0 < x < w and 0 < y < h in crop pixels).
+ *   dad3d_heatmap_targets  replaces HeatmapCoder.__call__ (data/coder.py:16-23) and np.uint8(255 * heatmap)
+ *     (flame_dataset.py:198): out_d [planes, S, S] uint8, every byte written, one CTA per plane.  Plane p with presence_d[p]
+ *     takes the window table_d [2 radius + 1]^2 (uint8(fp32(255 * fp32(g))) of the reference's gaussian_2d or
+ *     pointwise_gaussian_2d, built by the caller) at cell int(landmarks_d[p] // stride) (numpy's float32 divmod), placed
+ *     exactly as draw_gaussian's numpy slices place it (data/utils.py:51-70), negative and out-of-plane cells included. */
+DAD3D_API int dad3d_training_targets(const float* vertices_d, const float* model_view_d, const float* projection_d,
+                                     const int32_t* origins_d, const dad3d_roi* rois_d, int32_t B, int32_t V,
+                                     const int32_t* lm_index_d, const int32_t* lm_tri_d, const float* lm_bary_d, int32_t C,
+                                     int32_t img_size, float* keypoints_d, float* landmarks_d, float* landmarks_norm_d,
+                                     uint8_t* presence_d, dad3d_stream stream);
+DAD3D_API int dad3d_heatmap_targets(const float* landmarks_d, const uint8_t* presence_d, int32_t planes, int32_t S,
+                                    int32_t stride, const uint8_t* table_d, int32_t radius, uint8_t* out_d,
+                                    dad3d_stream stream);
+
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
 
