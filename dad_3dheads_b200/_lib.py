@@ -33,6 +33,15 @@ class Lighting(C.Structure):
                 ("light_pos", C.c_float * 3), ("view_pos", C.c_float * 3)]
 
 
+class KpGroup(C.Structure):
+    """dad3d_kp_group: one keypoint group of dad3d_keypoint_errors, passed in a host array."""
+    _fields_ = [("pred_d", C.c_void_p), ("target_d", C.c_void_p), ("index_d", C.c_void_p), ("presence_d", C.c_void_p),
+                ("box_w_d", C.c_void_p), ("box_h_d", C.c_void_p), ("pred_stride", C.c_int64), ("target_stride", C.c_int64),
+                ("presence_stride", C.c_int64), ("box_stride", C.c_int64), ("pred_scale", C.c_float),
+                ("target_scale", C.c_float), ("n", C.c_int32), ("k", C.c_int32), ("normalize", C.c_int32),
+                ("pad_", C.c_int32)]
+
+
 _lib = None
 
 # every symbol include/dad3d.h declares: (restype, argtypes)
@@ -147,12 +156,20 @@ SIGNATURES = {
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "dad3d_heatmap_targets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_void_p, C.c_void_p]),
+    "dad3d_iou_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                  C.c_void_p]),
+    "dad3d_keypoint_errors": (C.c_int, [C.POINTER(KpGroup), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "dad3d_metrics_reduce": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
+                                       C.c_int32, C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
 }
 
 DAD3D_LOSS_L1 = 0
 DAD3D_LOSS_L2 = 1
 DAD3D_LOSS_SMOOTH_L1 = 2
 DAD3D_VSUB_RECORD_FLOATS = 32
+DAD3D_METRIC_MAX_GROUPS = 4
+DAD3D_METRIC_MAX_THRESHOLDS = 4
 
 
 def load():

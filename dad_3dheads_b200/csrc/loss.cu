@@ -14,6 +14,7 @@
 
 #include "../../include/dad3d.h"
 #include "common.h"
+#include "reductions.cuh"
 
 struct dad3d_vsub {
   int32_t S = 0, V = 0, E = 0, device = 0;
@@ -26,9 +27,6 @@ struct dad3d_vsub {
 };
 
 namespace dad3d {
-
-constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
 
 // ---- criteria (nn.L1Loss / nn.MSELoss / nn.SmoothL1Loss(beta = 1) before their mean) ------------------------------------
 __device__ __forceinline__ float crit_value(int crit, float d) {
@@ -44,68 +42,6 @@ __device__ __forceinline__ float crit_grad(int crit, float d) {
   if (crit == DAD3D_LOSS_L2) return 2.f * d;
   return fabsf(d) < 1.f ? d : sg;
 }
-
-// ---- deterministic block reductions (256 threads; every thread gets the result) -------------------------------------
-template <int N>
-__device__ __forceinline__ void block_sum(float (&x)[N], float* sm /* [kWarps * N] */) {
-#pragma unroll
-  for (int k = 0; k < N; ++k)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x[k] += __shfl_xor_sync(0xffffffffu, x[k], o);
-  const int w = threadIdx.x >> 5;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int k = 0; k < N; ++k) sm[w * N + k] = x[k];
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    float s = 0.f;
-    for (int i = 0; i < kWarps; ++i) s += sm[i * N + k];
-    x[k] = s;
-  }
-}
-
-// (value, index) pairs: the extreme value, first index on ties -- the index torch's min / max over a dimension return.
-// A NaN never wins a comparison, so it cannot be selected; a head whose values are all NaN keeps the sentinel index.
-struct Ext {
-  float v;
-  int i;
-};
-template <bool MAX>
-__device__ __forceinline__ bool beats(float a, int ia, float b, int ib) {
-  return (MAX ? a > b : a < b) || (a == b && ia < ib);
-}
-template <bool MAX>
-__device__ __forceinline__ void take(Ext& e, float v, int i) {
-  if (beats<MAX>(v, i, e.v, e.i)) e = {v, i};
-}
-template <bool MAX, int N>
-__device__ __forceinline__ void block_ext(Ext (&x)[N], Ext* sm /* [kWarps * N] */) {
-#pragma unroll
-  for (int k = 0; k < N; ++k)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float v = __shfl_xor_sync(0xffffffffu, x[k].v, o);
-      const int i = __shfl_xor_sync(0xffffffffu, x[k].i, o);
-      take<MAX>(x[k], v, i);
-    }
-  const int w = threadIdx.x >> 5;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int k = 0; k < N; ++k) sm[w * N + k] = x[k];
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    Ext e = sm[k];
-    for (int i = 1; i < kWarps; ++i) take<MAX>(e, sm[i * N + k].v, sm[i * N + k].i);
-    x[k] = e;
-  }
-}
-
-template <bool MAX>
-__device__ __forceinline__ Ext ext_init() { return {MAX ? -INFINITY : INFINITY, INT_MAX}; }
 
 // ---- finalize: out = bias + sum_s coef_s * sum_b x[b * ld + s * sld], in fp64, in a fixed order ----------------------
 // coef_s = scale * w[s] / |set s| for the vertex-subset losses (w, off given), else scale.
@@ -131,55 +67,7 @@ finalize_kernel(const float* __restrict__ x, int B, int S, long long ld, int sld
 }
 
 // ---- heat-map IoU ---------------------------------------------------------------------------------------------------
-constexpr float kIouEps = 1e-6f;
-
-// sigmoid(x) and sigmoid'(x) = s (1 - s) = q / (1 + q)^2 with q = exp(-|x|): no cancellation in 1 - s, no overflow
-__device__ __forceinline__ void sigmoid2(float x, float& s, float& ds) {
-  const float q = expf(-fabsf(x));
-  const float r = 1.f / (1.f + q);
-  s = x >= 0.f ? r : q * r;
-  ds = q * r * r;
-}
-
-// (T + S) - I + eps: the reference's denominator, shared by forward and backward
-__device__ __forceinline__ float iou_den(float I, float T, float S) { return __fadd_rn(__fsub_rn(__fadd_rn(T, S), I), kIouEps); }
-
-__device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-// one block per (b, c) plane: stats [P, 4] = (I, T, S, iou)
-__global__ void __launch_bounds__(kThreads)
-iou_forward_kernel(const float* __restrict__ x, const float* __restrict__ t, int hw, float* __restrict__ stats) {
-  __shared__ float sm[kWarps * 3];
-  const size_t base = static_cast<size_t>(blockIdx.x) * hw;
-  const float* xp = x + base;
-  const float* tp = t + base;
-  float a[3] = {0.f, 0.f, 0.f};
-  auto add = [&](float xv, float tv) {
-    float s, ds;
-    sigmoid2(xv, s, ds);
-    a[0] = fmaf(s, tv, a[0]);
-    a[1] = fmaf(tv, tv, a[1]);
-    a[2] = fmaf(s, s, a[2]);
-  };
-  if ((hw & 3) == 0 && aligned16(xp) && aligned16(tp)) {
-    const float4* x4 = reinterpret_cast<const float4*>(xp);
-    const float4* t4 = reinterpret_cast<const float4*>(tp);
-#pragma unroll 4
-    for (int i = threadIdx.x; i < (hw >> 2); i += kThreads) {
-      const float4 xv = x4[i], tv = t4[i];
-      add(xv.x, tv.x); add(xv.y, tv.y); add(xv.z, tv.z); add(xv.w, tv.w);
-    }
-  } else {
-    for (int i = threadIdx.x; i < hw; i += kThreads) add(xp[i], tp[i]);
-  }
-  block_sum<3>(a, sm);
-  if (threadIdx.x == 0) {
-    float* st = stats + 4 * static_cast<size_t>(blockIdx.x);
-    st[0] = a[0]; st[1] = a[1]; st[2] = a[2];
-    st[3] = __fadd_rn(a[0], kIouEps) / iou_den(a[0], a[1], a[2]);
-  }
-}
-
+// The forward's per-plane statistics are iou_forward_kernel<true, float> (reductions.cuh), shared with the metrics.
 // d loss / d x = -g / P * (t D - N (2 s - t)) / D^2 * s (1 - s),  N = I + eps, D = T + S - I + eps
 __global__ void __launch_bounds__(kThreads)
 iou_backward_kernel(const float* __restrict__ x, const float* __restrict__ t, int hw, int P, const float* __restrict__ stats,
@@ -250,8 +138,6 @@ struct VsubRec {
   float sco, sg[3];
 };
 static_assert(sizeof(VsubRec) <= DAD3D_VSUB_RECORD_FLOATS * sizeof(float), "record size");
-
-__device__ __forceinline__ float centred(float v, float mn, float half) { return __fsub_rn(__fsub_rn(v, mn), half); }
 
 // one block per (head, set)
 template <int K, bool NORM>
@@ -446,7 +332,7 @@ int dad3d_iou_forward(const float* x_d, const float* t_d, int32_t planes, int32_
   DAD3D_REQUIRE(x_d && t_d && stats_d && loss_d, "null pointer");
   DAD3D_REQUIRE(planes >= 1 && hw >= 1, "shape");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  iou_forward_kernel<<<planes, kThreads, 0, stream>>>(x_d, t_d, hw, stats_d);
+  iou_forward_kernel<true, float><<<planes, kThreads, 0, stream>>>(x_d, t_d, hw, stats_d);
   count_launch();
   DAD3D_CUDA_OK(cudaGetLastError());
   finalize_kernel<<<1, kThreads, 0, stream>>>(stats_d + 3, planes, 1, 4, 0, nullptr, nullptr, -1.0 / planes, 1.0, loss_d);

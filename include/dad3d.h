@@ -527,6 +527,47 @@ DAD3D_API int dad3d_heatmap_targets(const float* landmarks_d, const uint8_t* pre
                                     int32_t stride, const uint8_t* table_d, int32_t radius, uint8_t* out_d,
                                     dad3d_stream stream);
 
+/* ---- training metrics: the metric block of FlameLightningModel._step_fn (train/flame_lightning_model.py:299-357) ------
+ * Per-plane and per-head partial results, then one reduction in a fixed order (fp64 sums, integer counts; no
+ * floating-point atomics).  Nothing synchronises with the host, so the calls capture in a CUDA graph.  Float inputs are
+ * contiguous fp32 unless a stride says otherwise.
+ *   dad3d_iou_stats  the per-plane statistics of soft_iou (metrics/iou.py:15-31), with the kernel dad3d_iou_forward
+ *     runs: x_d [planes, hw] probabilities (logits = 0) or logits (logits = 1, s = sigmoid(x)); t_d fp32 or, with
+ *     target_u8 = 1, uint8 read as fp32(u) / 255 (uint8_to_float32, model/flame.py:232-236).  stats_d [planes, 4] =
+ *     (I = sum s t, T = sum t^2, S = sum s^2, iou at eps 1e-6) (1 kernel).
+ *   dad3d_keypoint_errors  one CTA per (head, group): err = mean_n |p_n - t_n|_2 over the group's n keypoints of dimension
+ *     k (2 or 3) and norm = sqrt(fp32(w * h)) (int32 product, keypoints.py:19-52) or 2.0 without a box; records_d
+ *     [B, G, 2] = (err, norm).  Keypoint j of head b is row index_d[j] (or j) of pred_d + b * pred_stride and of
+ *     target_d + b * target_stride; with presence_d, prediction fp32(fp32(p * pred_scale) * m) and target
+ *     fp32(fp32(t * m) * target_scale), m = presence_d[b * presence_stride + j] (0 or 1), the order of the step's products
+ *     (flame_lightning_model.py:316-319); with normalize, normalize_to_cube (model/utils.py:55-68) of both operands over
+ *     the group's keypoints (1 kernel).
+ *   dad3d_metrics_reduce  one CTA: values_d = [mean iou (when stats_d is given)] then per group [nme_scale * mean_b(err /
+ *     norm), then per threshold count_b(err < fp32(thr * norm)) / B (err > ... when below = 0)].  per_head_d [B, G] (or
+ *     NULL) gets err / norm.  With epoch_d [n_values + 1] fp64: epoch_d[i] += values_d[i] * weight, epoch_d[n_values] +=
+ *     weight, and epoch_values_d[i] = epoch_d[i] / epoch_d[n_values] (1 kernel). */
+#define DAD3D_METRIC_MAX_GROUPS 4
+#define DAD3D_METRIC_MAX_THRESHOLDS 4
+typedef struct dad3d_kp_group {
+  const float* pred_d;
+  const float* target_d;
+  const int32_t* index_d;
+  const uint8_t* presence_d;
+  const int32_t* box_w_d; /* box widths and heights (NULL: norm 2.0), element b at b * box_stride */
+  const int32_t* box_h_d;
+  int64_t pred_stride, target_stride, presence_stride, box_stride;
+  float pred_scale, target_scale;
+  int32_t n, k, normalize, pad_;
+} dad3d_kp_group;
+DAD3D_API int dad3d_iou_stats(const float* x_d, const void* t_d, int32_t target_u8, int32_t logits, int32_t planes,
+                              int32_t hw, float* stats_d, dad3d_stream stream);
+DAD3D_API int dad3d_keypoint_errors(const dad3d_kp_group* groups_h, int32_t G, int32_t B, float* records_d,
+                                    dad3d_stream stream);
+DAD3D_API int dad3d_metrics_reduce(const float* stats_d, int32_t planes, float eps, const float* records_d, int32_t B,
+                                   int32_t G, float nme_scale, int32_t below, const float* thresholds_h, int32_t n_thresholds,
+                                   double weight, float* values_d, float* per_head_d, double* epoch_d,
+                                   float* epoch_values_d, dad3d_stream stream);
+
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
 
