@@ -29,17 +29,27 @@ struct dad3d_vsub {
 namespace dad3d {
 
 // ---- criteria (nn.L1Loss / nn.MSELoss / nn.SmoothL1Loss(beta = 1) before their mean) ------------------------------------
+// Every fp32 and fp64 site nvcc could contract is written with an explicit rounding, in the form nvcc already chose (the
+// SASS is unchanged), so tests/loss_model.py can restate each kernel exactly.
 __device__ __forceinline__ float crit_value(int crit, float d) {
   const float a = fabsf(d);
   if (crit == DAD3D_LOSS_L1) return a;
-  if (crit == DAD3D_LOSS_L2) return d * d;
-  return a < 1.f ? 0.5f * d * d : a - 0.5f;
+  if (crit == DAD3D_LOSS_L2) return __fmul_rn(d, d);
+  return a < 1.f ? __fmul_rn(__fmul_rn(0.5f, d), d) : __fsub_rn(a, 0.5f);
+}
+
+// acc + crit_value(crit, d): l2's square is fused into the sum; the other criteria round their value, then the sum
+__device__ __forceinline__ float crit_accum(int crit, float d, float acc) {
+  const float a = fabsf(d);
+  if (crit == DAD3D_LOSS_L1) return __fadd_rn(acc, a);
+  if (crit == DAD3D_LOSS_L2) return __fmaf_rn(d, d, acc);
+  return __fadd_rn(acc, a < 1.f ? __fmul_rn(__fmul_rn(0.5f, d), d) : __fsub_rn(a, 0.5f));
 }
 
 __device__ __forceinline__ float crit_grad(int crit, float d) {
   const float sg = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
   if (crit == DAD3D_LOSS_L1) return sg;
-  if (crit == DAD3D_LOSS_L2) return 2.f * d;
+  if (crit == DAD3D_LOSS_L2) return __fadd_rn(d, d);      // 2 d, exact
   return fabsf(d) < 1.f ? d : sg;
 }
 
@@ -52,16 +62,17 @@ finalize_kernel(const float* __restrict__ x, int B, int S, long long ld, int sld
   double total = bias;
   for (int s = 0; s < S; ++s) {
     double acc = 0.0;
-    for (int b = threadIdx.x; b < B; b += kThreads) acc += static_cast<double>(x[b * ld + static_cast<long long>(s) * sld]);
+    for (int b = threadIdx.x; b < B; b += kThreads)
+      acc = __dadd_rn(acc, static_cast<double>(x[b * ld + static_cast<long long>(s) * sld]));
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    for (int o = 16; o > 0; o >>= 1) acc = __dadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
     __syncthreads();
     if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = acc;
     __syncthreads();
     double sum = 0.0;
-    for (int i = 0; i < kWarps; ++i) sum += sm[i];
-    const double coef = w ? scale * static_cast<double>(w[s]) / static_cast<double>(off[s + 1] - off[s]) : scale;
-    total += coef * sum;
+    for (int i = 0; i < kWarps; ++i) sum = __dadd_rn(sum, sm[i]);
+    const double coef = w ? __dmul_rn(scale, static_cast<double>(w[s])) / static_cast<double>(off[s + 1] - off[s]) : scale;
+    total = __fma_rn(coef, sum, total);
   }
   if (threadIdx.x == 0) *out = static_cast<float>(total);
 }
@@ -82,7 +93,7 @@ iou_backward_kernel(const float* __restrict__ x, const float* __restrict__ t, in
   auto grad = [&](float xv, float tv) {
     float s, ds;
     sigmoid2(xv, s, ds);
-    return coef * (tv * D - N * (2.f * s - tv)) * ds;
+    return __fmul_rn(__fmul_rn(coef, __fmaf_rn(tv, D, -__fmul_rn(N, __fsub_rn(__fadd_rn(s, s), tv)))), ds);
   };
   if ((hw & 3) == 0 && aligned16(xp) && aligned16(tp) && aligned16(gp)) {
     const float4* x4 = reinterpret_cast<const float4*>(xp);
@@ -108,7 +119,7 @@ __global__ void lmk_forward_kernel(const float* __restrict__ p, const float* __r
     const size_t i = static_cast<size_t>(b) * N + n;
     const float mp = pm[i], mt = tm[i];
 #pragma unroll
-    for (int c = 0; c < 2; ++c) acc += crit_value(crit, p[2 * i + c] * mp - t[2 * i + c] * mt);
+    for (int c = 0; c < 2; ++c) acc += crit_value(crit, __fmaf_rn(p[2 * i + c], mp, -__fmul_rn(t[2 * i + c], mt)));
   }
   partial[b] = static_cast<float>(acc);
 }
@@ -121,7 +132,7 @@ __global__ void lmk_backward_kernel(const float* __restrict__ p, const float* __
   const long long i = e >> 1;
   const float scale = *grad_out / (2.f * static_cast<float>(B) * static_cast<float>(N));
   const float mp = pm[i];
-  gp[e] = scale * crit_grad(crit, p[e] * mp - t[e] * tm[i]) * mp;
+  gp[e] = __fmul_rn(__fmul_rn(scale, crit_grad(crit, __fmaf_rn(p[e], mp, -__fmul_rn(t[e], tm[i])))), mp);
 }
 
 // ---- vertex-subset losses ---------------------------------------------------------------------------------------------
@@ -157,7 +168,7 @@ vsub_forward_kernel(const float* __restrict__ v, const float* __restrict__ t, in
     for (int j = threadIdx.x; j < n; j += kThreads) {
       const size_t q = static_cast<size_t>(I[j]) * K;
 #pragma unroll
-      for (int c = 0; c < K; ++c) a[0] += crit_value(crit, vb[q + c] - tb[q + c]);
+      for (int c = 0; c < K; ++c) a[0] = crit_accum(crit, vb[q + c] - tb[q + c], a[0]);
     }
     block_sum<1>(a, smf);
     if (threadIdx.x == 0) R->loss = a[0];
@@ -212,7 +223,7 @@ vsub_forward_kernel(const float* __restrict__ v, const float* __restrict__ t, in
         const float w = centred(tb[q + c], lo[K + c].v, half[K + c]) / tM;
         const float d = u - w;
         const float cd = crit_grad(crit, d);
-        a[0] += crit_value(crit, d);
+        a[0] = crit_accum(crit, d, a[0]);
         a[1] = fmaf(cd, u, a[1]);
         a[2 + c] += cd;
       }
@@ -280,7 +291,7 @@ vsub_backward_kernel(const float* __restrict__ v, const float* __restrict__ t, i
       }
     } else {
 #pragma unroll
-      for (int c = 0; c < K; ++c) acc[c] += coef * crit_grad(crit, x[c] - y[c]);
+      for (int c = 0; c < K; ++c) acc[c] = __fmaf_rn(coef, crit_grad(crit, x[c] - y[c]), acc[c]);
     }
   }
 #pragma unroll
