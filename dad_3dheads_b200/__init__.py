@@ -6,9 +6,11 @@ compute classes without the built library, or calling them without a Hopper GPU,
 """
 from .flame import FLAME_CONSTS, FlameParams, FLAMELayer  # noqa: F401
 from .head_mesh import HeadMesh  # noqa: F401
+from .heads import FlameHeads, FrozenBackboneRegression  # noqa: F401
 from .losses import IoULoss, LandmarksLossWVisibility, ReprojectionLoss, Vertices3DLoss  # noqa: F401
 from .metrics import FlameStepMetrics  # noqa: F401
 from .training_data import FlameBatchBuilder, FlameDataset  # noqa: F401
 
-__all__ = ["FLAME_CONSTS", "FlameBatchBuilder", "FlameDataset", "FlameParams", "FlameStepMetrics", "FLAMELayer", "HeadMesh", "IoULoss",
+__all__ = ["FLAME_CONSTS", "FlameBatchBuilder", "FlameDataset", "FlameHeads", "FlameParams", "FlameStepMetrics", "FLAMELayer",
+           "FrozenBackboneRegression", "HeadMesh", "IoULoss",
            "LandmarksLossWVisibility", "ReprojectionLoss", "Vertices3DLoss"]

@@ -162,6 +162,15 @@ SIGNATURES = {
     "dad3d_metrics_reduce": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                        C.c_int32, C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
+    "dad3d_encoder_features": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_size_t, C.c_void_p]),
+    "dad3d_heads_workspace_bytes": (C.c_size_t, [C.c_int32]),
+    "dad3d_heads_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                                      C.c_int32, C.c_double, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_heads_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_float, C.c_int32,
+                                       C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 DAD3D_LOSS_L1 = 0

@@ -693,9 +693,10 @@ int launch_conv(dad3d_encoder* enc, const Step& s, cudaStream_t stream) {
   return DAD3D_OK;
 }
 
-// one step of the plan, as dad3d_encoder_forward runs it (the single-step test hook runs the same code)
+// one step of the plan, as dad3d_encoder_forward runs it (the single-step test hook runs the same code); with features_d
+// the GAP step also stores its fp32 means there
 int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* params_d, float* landmarks_d, float* heatmap_d,
-             cudaStream_t stream) {
+             cudaStream_t stream, float* features_d = nullptr) {
   const Plan& plan = *enc->plan;
   const int B = plan.B;
   auto T = [&](int id) -> const TensorInfo& { return plan.tensors[id]; };
@@ -768,9 +769,9 @@ int run_step(dad3d_encoder* enc, const Step& s, const float* images_d, float* pa
     case kGap: {
       const TensorInfo& ti = T(s.in);
       const TensorInfo& to = T(s.out);
-      gap_kernel<<<B * (ti.C / 64), 256, 0, stream>>>(view(s.in), B, ti.H * ti.W, ti.C,
-                                                           reinterpret_cast<uint16_t*>(to.ptr), to.plane_elems(), to.planes,
-                                                           enc->fp16);
+      auto* gap = features_d ? gap_kernel<true> : gap_kernel<false>;
+      gap<<<B * (ti.C / 64), 256, 0, stream>>>(view(s.in), B, ti.H * ti.W, ti.C, reinterpret_cast<uint16_t*>(to.ptr),
+                                                to.plane_elems(), to.planes, enc->fp16, features_d);
       count_launch();
       break;
     }
@@ -995,6 +996,28 @@ int dad3d_encoder_forward(dad3d_encoder* enc, const float* images_d, int32_t B, 
   for (const Step& s : enc->plan->steps) {
     int rc = run_step(enc, s, images_d, params_d, landmarks_d, heatmap_d, stream);
     if (rc != DAD3D_OK) return rc;
+  }
+  DAD3D_CUDA_OK(cudaGetLastError());
+  return DAD3D_OK;
+}
+
+int dad3d_encoder_features(dad3d_encoder* enc, const float* images_d, int32_t B, float* features_d, float* heatmap_d,
+                           void* workspace_d, size_t workspace_bytes, dad3d_stream stream_) {
+  DAD3D_REQUIRE(enc, "null handle");
+  if (B == 0) return DAD3D_OK;
+  DAD3D_REQUIRE(B > 0 && images_d && features_d && workspace_d, "null pointer / batch");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!enc->plan || enc->plan->B != B || enc->plan->ws != workspace_d || enc->plan->ws_bytes != workspace_bytes) {
+    int rc = make_plan(enc, B, workspace_d, workspace_bytes, false, nullptr);
+    if (rc != DAD3D_OK) return rc;
+  }
+  // the forward's steps up to the pool, then only the heat-map export: mlp1, mlp2 and the head epilogue are skipped
+  bool pooled = false;
+  for (const Step& s : enc->plan->steps) {
+    if (pooled && s.kind != kHeatExport) continue;
+    int rc = run_step(enc, s, images_d, nullptr, nullptr, heatmap_d, stream, features_d);
+    if (rc != DAD3D_OK) return rc;
+    pooled = pooled || s.kind == kGap;
   }
   DAD3D_CUDA_OK(cudaGetLastError());
   return DAD3D_OK;

@@ -507,9 +507,12 @@ __global__ void fusion_concat_kernel(ActView x, int Cx, const float* __restrict_
 // ------------------------------------------------------------------------------------------------ GAP
 // adaptive_avg_pool2d(., 1): [B,HW,C] -> [B,C] pieces.  thread = 8 channels of an image.
 // block = one image x 8 channel groups (64 channels); thread = (pixel slice 0..31, channel group): pixels slice, slice+32, ...
+// kF32Out also stores the fp32 means [B,C] to means (the frozen-backbone features), the values the pieces are split from.
 constexpr int kGapSlices = 32;
+template <bool kF32Out>
 __global__ void __launch_bounds__(256)
-gap_kernel(ActView x, int B, int HW, int C, uint16_t* __restrict__ out, long long out_plane, int planes, int fp16) {
+gap_kernel(ActView x, int B, int HW, int C, uint16_t* __restrict__ out, long long out_plane, int planes, int fp16,
+           float* __restrict__ means) {
   __shared__ float red[kGapSlices][8][9];
   const int cgs = C / 8;
   const int blocks_per_img = cgs / 8;
@@ -532,6 +535,7 @@ gap_kernel(ActView x, int B, int HW, int C, uint16_t* __restrict__ out, long lon
     float sum = 0.f;
     for (int sl = 0; sl < kGapSlices; ++sl) sum += red[sl][g][j];
     red[0][g][j] = sum / static_cast<float>(HW);
+    if (kF32Out) means[static_cast<long long>(b) * C + (blockIdx.x % blocks_per_img) * 64 + threadIdx.x] = red[0][g][j];
   }
   __syncthreads();
   if (threadIdx.x < 8) {

@@ -271,6 +271,16 @@ class Dad3dEncoder:
                                                         ptr(heatmap), torch.cuda.current_stream(self.device).cuda_stream),
                        "dad3d_encoder_run_steps")
 
+    def _workspace(self, B: int) -> Tensor:
+        """The scratch buffer for a batch of B, grown (and ws_generation bumped) when the plan needs more."""
+        need = int(self.lib.dad3d_encoder_workspace_bytes(self._h, B))
+        if need == 0:
+            _lib.check(-1, "dad3d_encoder_workspace_bytes")
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            self.ws_generation += 1
+        return self._ws
+
     def forward_raw(self, x: Tensor, want_heatmap: Optional[bool] = None):
         """x: [B,3,256,256] fp32 CUDA.  -> (params [B,413], landmarks [B,68,2], heatmap [B,68,64,64] | None)."""
         assert x.ndim == 4 and x.shape[1:] == (3, 256, 256), x.shape
@@ -282,19 +292,34 @@ class Dad3dEncoder:
         heat = torch.empty(B, 68, 64, 64, dtype=torch.float32, device=self.device) if want_heatmap else None
         if B == 0:
             return params, lms, heat
-        need = int(self.lib.dad3d_encoder_workspace_bytes(self._h, B))
-        if need == 0:
-            _lib.check(-1, "dad3d_encoder_workspace_bytes")
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
-            self.ws_generation += 1
+        ws = self._workspace(B)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.dad3d_encoder_forward(self._h, x.data_ptr(), B, params.data_ptr(), lms.data_ptr(),
                                                       heat.data_ptr() if heat is not None else None,
-                                                      self._ws.data_ptr(), self._ws.numel(),
+                                                      ws.data_ptr(), ws.numel(),
                                                       torch.cuda.current_stream(self.device).cuda_stream),
                        "dad3d_encoder_forward")
         return params, lms, heat
+
+    def features(self, x: Tensor, want_heatmap: Optional[bool] = None):
+        """x: [B,3,256,256] fp32 CUDA -> (features [B,2048], heatmap [B,68,64,64] | None): the pooled stage-4 map
+        (F.adaptive_avg_pool2d(fmap, 1)) that the regression heads read, from the forward's steps up to the pool."""
+        assert x.ndim == 4 and x.shape[1:] == (3, 256, 256), x.shape
+        x = x.to(self.device, torch.float32).contiguous()
+        B = x.shape[0]
+        want_heatmap = self.want_heatmap if want_heatmap is None else want_heatmap
+        feats = torch.empty(B, 2048, dtype=torch.float32, device=self.device)
+        heat = torch.empty(B, 68, 64, 64, dtype=torch.float32, device=self.device) if want_heatmap else None
+        if B == 0:
+            return feats, heat
+        ws = self._workspace(B)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.dad3d_encoder_features(self._h, x.data_ptr(), B, feats.data_ptr(),
+                                                       heat.data_ptr() if heat is not None else None,
+                                                       ws.data_ptr(), ws.numel(),
+                                                       torch.cuda.current_stream(self.device).cuda_stream),
+                       "dad3d_encoder_features")
+        return feats, heat
 
     def __call__(self, x: Tensor) -> Dict[str, Tensor]:
         params, lms, heat = self.forward_raw(x)

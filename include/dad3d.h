@@ -206,6 +206,13 @@ DAD3D_API int dad3d_encoder_forward(dad3d_encoder* enc, const float* images_d, i
                                     float* landmarks_d, float* heatmap_d, void* workspace_d, size_t workspace_bytes,
                                     dad3d_stream stream);
 
+/* The frozen-backbone features of DAD-3DNet's regression heads: the forward's steps through the global average pool
+ * (F.adaptive_avg_pool2d(fmap, 1), flame_regression.py:57), without mlp1 / mlp2 / the head epilogue.  features_d [B,2048]
+ * fp32 gets the pool's fp32 means (the values the forward splits into operand pieces); heatmap_d as in
+ * dad3d_encoder_forward (NULL: none).  Same plan, workspace size and launches as the forward up to the pool. */
+DAD3D_API int dad3d_encoder_features(dad3d_encoder* enc, const float* images_d, int32_t B, float* features_d,
+                                     float* heatmap_d, void* workspace_d, size_t workspace_bytes, dad3d_stream stream);
+
 /* ---- device-side pre-processing (SURVEY §8f "next" row 2) --------------------------------------------------------------
  * dad3d_preprocess replaces FaceMeshPredictor._transform + _array_to_batch (predictor.py:85-89,195-203: albumentations
  *   LongestMaxSize -> PadIfNeeded -> Normalize -> HWC->CHW) for one image: image_d [H,W,3] uint8 RGB (device) ->
@@ -567,6 +574,37 @@ DAD3D_API int dad3d_metrics_reduce(const float* stats_d, int32_t planes, float e
                                    int32_t G, float nme_scale, int32_t below, const float* thresholds_h, int32_t n_thresholds,
                                    double weight, float* values_d, float* per_head_d, double* epoch_d,
                                    float* epoch_values_d, dad3d_stream stream);
+
+/* ---- DAD-3DNet's regression heads, trainable (csrc/heads.cu) -----------------------------------------------------------
+ * The three ClassificationHeads (flame_regression.py:45-59: Linear 2048->512, ReLU, Dropout(0.3), Linear 512->{403, 10,
+ * 136}) and their epilogue (:96-100: tanh * limit_value on shape, identity on pose, ReLU on the landmarks), fp32 on the CUDA
+ * cores, every sum in a fixed order (bit-reproducible; no floating-point atomics).  Packed weights: w1_d [1536,2048] (rows
+ * shape | pose | landmarks of logit_image.0), b1_d [1536], w2_d [549,512] (rows 0-402 shape, 403-412 pose, 413-548
+ * landmarks of logit_image.3; row r reads the 512-wide hidden block of its head), b2_d [549].
+ *   B is 1 to 524280 (8 x 65535).  p is the dropout probability as a double (a Python float), so fp32(1 - p) and
+ *   fp32(1 / (1 - p)) round from fp64 as torch's do.
+ *   dad3d_heads_workspace_bytes  scratch either call needs at batch B.
+ *   dad3d_heads_forward  features_d [B,2048] -> params_d [B,413] = [tanh(o) * limit | o] (OUTPUT_3DMM_PARAMS), landmarks_d
+ *     [B,68,2] = relu(o) (OUTPUT_2D_LANDMARKS).  Saved for the backward: h_d [B,1536] = relu(f w1^T + b1), d_d [B,1536] the
+ *     dropped activations, mask_d uint32 [B,48] keep bits (bit j of word w: column 32 w + j), y_d [B,403] = tanh(o), obits_d
+ *     uint32 [B,18] o > 0 bits of all 549 columns.  train = 1: keep iff fp32(x >> 8) * 2^-24 < fp32(1 - p) for word 0 x of
+ *     Philox4x32-10 at key (seed lo, seed hi) and counter (*counter_d lo, hi, row * 1536 + column, 0); kept values are
+ *     h * fp32(1 / (1 - p)) (torch's dropout arithmetic); the last kernel adds 1 to *counter_d, so a replayed graph draws a
+ *     fresh mask.  train = 0: no mask (all bits set), scale 1, counter_d unused (4 kernels).
+ *   dad3d_heads_backward  dparams_d [B,413], dlandmarks_d [B,136] -> dw1_d [1536,2048], db1_d [1536], dw2_d [549,512] (packed
+ *     as w2_d), db2_d [549]; no gradient for the features.  train and p as in the forward that saved h_d ... obits_d
+ *     (4 kernels). */
+DAD3D_API size_t dad3d_heads_workspace_bytes(int32_t B);
+DAD3D_API int dad3d_heads_forward(const float* features_d, int32_t B, const float* w1_d, const float* b1_d,
+                                  const float* w2_d, const float* b2_d, float limit, int32_t train, double p, uint64_t seed,
+                                  unsigned long long* counter_d, float* params_d, float* landmarks_d, float* h_d,
+                                  float* d_d, uint32_t* mask_d, float* y_d, uint32_t* obits_d, void* workspace_d,
+                                  size_t workspace_bytes, dad3d_stream stream);
+DAD3D_API int dad3d_heads_backward(const float* dparams_d, const float* dlandmarks_d, const float* features_d, int32_t B,
+                                   const float* w2_d, float limit, int32_t train, double p, const float* h_d,
+                                   const float* d_d, const uint32_t* mask_d, const float* y_d, const uint32_t* obits_d,
+                                   float* dw1_d, float* db1_d, float* dw2_d, float* db2_d, void* workspace_d,
+                                   size_t workspace_bytes, dad3d_stream stream);
 
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
