@@ -171,6 +171,12 @@ SIGNATURES = {
     "dad3d_heads_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_float, C.c_int32,
                                        C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dad3d_uv_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                  C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
+    "dad3d_uv_destroy": (None, [C.c_void_p]),
+    "dad3d_uv_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int32]),
+    "dad3d_uv_texture": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                   C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 DAD3D_LOSS_L1 = 0

@@ -29,6 +29,7 @@ from .head_mesh import HeadMesh
 from . import overlay as overlay_ops
 from .overlay import OVERLAY_KINDS
 from .rasterizer import LitRenderer, PnccRenderer
+from .uv_texture import UvTextureTable, uv_textures
 
 logger = logging.getLogger(__name__)
 ROI_RECORD_BYTES = 72                                # sizeof(dad3d_roi), include/dad3d.h
@@ -109,8 +110,9 @@ class StepOptions:
 
     The fields take ``predict_batch``'s arguments.  After construction ``render``, ``frame_render`` and ``overlay`` are
     tuples in the order of RENDER_KEYS, FRAME_RENDER_KEYS and OVERLAY_KINDS, ``rpy`` is a bool, ``rois`` is None (no
-    boxes) or the number of boxes per step, and ``extend`` is the four fractions of :func:`extend_sides` with boxes and
-    None without them (where it is ignored).  Unknown names and unsupported combinations raise ValueError."""
+    boxes) or the number of boxes per step, ``extend`` is the four fractions of :func:`extend_sides` with boxes and
+    None without them (where it is ignored), and ``uv_texture`` is None, a table path (str) or a :class:`UvTextureTable`.
+    Unknown names and unsupported combinations raise ValueError."""
     landmark_subset: Optional[str] = "445"
     to_2d: bool = True
     fast_decode: bool = True
@@ -120,6 +122,7 @@ class StepOptions:
     rpy: bool = False
     rois: Optional[int] = None
     extend: Any = 0.0
+    uv_texture: Any = None
 
     def __post_init__(self):
         render = _names("render", self.render, RENDER_KEYS, "maps")
@@ -136,9 +139,21 @@ class StepOptions:
             raise ValueError("overlay needs boxes: it draws into copies of the frames, which the no-box path does not have")
         if render and boxes:
             raise ValueError("render is not supported together with boxes")
+        uv = self.uv_texture
+        if uv is not None:
+            if not boxes:
+                raise ValueError("uv_texture needs boxes: it samples each box's frame, which the no-box path does not have")
+            if self.to_2d:
+                raise ValueError("uv_texture needs to_2d=False: the texture's visibility test takes the projected vertices "
+                                 "with their depth")
+            if isinstance(uv, os.PathLike):
+                uv = os.fspath(uv)
+            if not isinstance(uv, (str, UvTextureTable)):
+                raise ValueError(f"uv_texture: a path to texture_data.npy or a UvTextureTable, got {type(uv).__name__}")
         canonical = dict(to_2d=bool(self.to_2d), fast_decode=bool(self.fast_decode), render=render,
                          frame_render=frame_render, overlay=overlay, rpy=bool(self.rpy),
-                         rois=int(self.rois) if boxes else None, extend=extend_sides(self.extend) if boxes else None)
+                         rois=int(self.rois) if boxes else None, extend=extend_sides(self.extend) if boxes else None,
+                         uv_texture=uv)
         for name, value in canonical.items():
             object.__setattr__(self, name, value)
 
@@ -189,6 +204,7 @@ class FaceMeshPredictor:
         self._graphs: Dict[Any, CapturedStep] = {}
         self._renderer: Optional[PnccRenderer] = None
         self._lit_renderer: Optional[LitRenderer] = None
+        self._uv_tables: Dict[str, UvTextureTable] = {}
 
     # ------------------------------------------------------------------ reference single-image API
     def __call__(self, x: Any) -> Any:
@@ -355,6 +371,17 @@ class FaceMeshPredictor:
             self._lit_renderer = LitRenderer(self.device)
         return self._lit_renderer
 
+    def _uv_table(self, spec) -> UvTextureTable:
+        """StepOptions.uv_texture -> the table on this predictor's device (a path is loaded once and kept)."""
+        if isinstance(spec, UvTextureTable):
+            if spec.device != self.device:
+                raise ValueError(f"uv_texture: the table is on {spec.device}, the predictor on {self.device}")
+            return spec
+        table = self._uv_tables.get(spec)
+        if table is None:
+            table = self._uv_tables[spec] = UvTextureTable.load(spec, self.device)
+        return table
+
     def _check_rois(self, frames, boxes, frame_index) -> Tuple[Tensor, Optional[Tensor]]:
         """Validates the frames + boxes arguments before anything is launched -> (boxes, frame_index) as tensors."""
         if not (isinstance(frames, Tensor) and frames.dtype == torch.uint8 and frames.ndim == 4 and frames.shape[3] == 3):
@@ -465,11 +492,15 @@ class FaceMeshPredictor:
                 subset = "191" if k == "191_landmarks" else "565"
                 overlay_ops.draw_points(img, proj.contiguous(), rois, self._landmark_index(subset))
             out[f"frame_{k}"] = img
+        if opts.uv_texture is not None:
+            out["uv_texture"] = uv_textures(self._uv_table(opts.uv_texture), frames, proj.contiguous(),
+                                            fields[:, 4].contiguous(), out["valid"])
         return out
 
     def predict_batch(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                       fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                      extend=0.0, frame_render=None, overlay=None, rpy: bool = False) -> Dict[str, Tensor]:
+                      extend=0.0, frame_render=None, overlay=None, rpy: bool = False,
+                      uv_texture=None) -> Dict[str, Tensor]:
         """images: [B,3,256,256] fp32 already letter-boxed + normalised, or raw RGB as the reference's ``__call__`` takes it:
         one [B,H,W,3] uint8 tensor / a list of HxWx3 uint8 images (letter-boxed + normalised on the GPU, bit-identical to
         the reference's albumentations pipeline); host or device.  All outputs stay on the GPU:
@@ -525,13 +556,19 @@ class FaceMeshPredictor:
         end point of the subset's edges blanks that box's whole wireframe), and the pose of a box whose crop is under 200 px high (thickness 0, which cv2.arrowedLine refuses;
         its "rpy" is still written).  A whole image is the box [0, 0, W, H] with ``extend=0``.
 
+        ``uv_texture`` (with ``boxes`` and ``to_2d=False``): the path of the reference's ``inference/texture_data.npy``
+        (loaded once per path) or a :class:`~dad_3dheads_b200.uv_texture.UvTextureTable` on this predictor's device adds
+        "uv_texture" [R,512,512,3] uint8: each box's texture, byte for byte the reference's
+        ``UVTextureCreator._compute_texture_map(frame, Mesh(projected_vertices[r], faces))`` on its frame
+        (:func:`~dad_3dheads_b200.uv_texture.uv_textures` on the step's own vertices); all zero for an invalid box.
+
         ``rpy=True`` adds "rpy" [B|R,3] float64, (roll, pitch, yaw) in degrees: ``calculate_rpy`` on each head's parameters
         (the reference computes head 0 only), to ~1e-12 degrees away from gimbal lock (scipy's SVD polar factor of the
         fp32 rotation is taken by Newton steps on the device).  With boxes, the rotation is that of the crop: the read-back does not change it."""
         if boxes is not None:
             boxes, frame_index = self._check_rois(images, boxes, frame_index)
         opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy,
-                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend)
+                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend, uv_texture=uv_texture)
         return self._step(images, opts, boxes, frame_index)
 
     def _ws_generation(self):
@@ -541,7 +578,8 @@ class FaceMeshPredictor:
 
     def predict_batch_graphed(self, images: Tensor, landmark_subset: Optional[str] = "445", to_2d: bool = True,
                               fast_decode: bool = True, render=None, boxes=None, frame_index=None,
-                              extend=0.0, frame_render=None, overlay=None, rpy: bool = False) -> Dict[str, Tensor]:
+                              extend=0.0, frame_render=None, overlay=None, rpy: bool = False,
+                      uv_texture=None) -> Dict[str, Tensor]:
         """:meth:`predict_batch` replayed from a CUDA graph (one graph per input shape / dtype / option set): the ~110 kernel
         launches of a step become one graph launch, which removes the launch gaps between the many sub-20 us layers.
         ``images`` is copied into the graph's static input buffer (host or device source); the returned tensors are the
@@ -552,12 +590,13 @@ class FaceMeshPredictor:
         re-captured before it is replayed again (``_ws_generation``), so a stale pointer is never dereferenced.
 
         With ``boxes`` (see :meth:`predict_batch`) the boxes and frame indices are copied into static buffers as well: one
-        graph serves every box set of the same frame shape, box count, ``extend``, ``frame_render`` and ``overlay``."""
+        graph serves every box set of the same frame shape, box count, ``extend``, ``frame_render``, ``overlay`` and
+        ``uv_texture``."""
         assert isinstance(images, Tensor), "the graphed path takes one tensor ([B,3,S,S] fp32 or [B,H,W,3] uint8)"
         if boxes is not None:
             boxes, frame_index = self._check_rois(images, boxes, frame_index)
         opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy,
-                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend)
+                           rois=None if boxes is None else int(boxes.shape[0]), extend=extend, uv_texture=uv_texture)
         key = (opts, tuple(images.shape), images.dtype)
         step = self._graphs.get(key)
         if step is None:
@@ -641,16 +680,17 @@ class BatchStream:
     ``keys`` to have them copied to the host like the other outputs.  With ``rois=R`` each batch is frames plus R boxes
     (``predict_batch``'s ``boxes``): ``submit(frames, boxes=, frame_index=)`` copies the boxes on the copy stream together with
     the frames; "crop_boxes" and "valid" may be listed in ``keys``, and with ``frame_render`` (passed to ``predict_batch``)
-    the "frame_<map>" outputs too; likewise "frame_<kind>" with ``overlay`` and "rpy" with ``rpy=True``.
+    the "frame_<map>" outputs too; likewise "frame_<kind>" with ``overlay``, "rpy" with ``rpy=True`` and "uv_texture"
+    with ``uv_texture``.
     """
 
     def __init__(self, predictor: FaceMeshPredictor, shape, dtype=torch.uint8, landmark_subset: Optional[str] = "445",
                  to_2d: bool = True, fast_decode: bool = True, depth: int = 2, render=None,
                  keys=("3dmm_params", "points", "3d_vertices", "landmarks_445"), host_results: bool = True,
                  group=None, gather_keys=("3dmm_params", "3d_vertices", "landmarks_445"), comm=None, rois=None,
-                 extend=0.0, frame_render=None, overlay=None, rpy: bool = False):
+                 extend=0.0, frame_render=None, overlay=None, rpy: bool = False, uv_texture=None):
         self.opts = StepOptions(landmark_subset, to_2d, fast_decode, render, frame_render, overlay, rpy, rois=rois,
-                                extend=extend)
+                                extend=extend, uv_texture=uv_texture)
         self.pred = predictor
         dev = predictor.device
         self.device = dev

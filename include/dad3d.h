@@ -606,6 +606,32 @@ DAD3D_API int dad3d_heads_backward(const float* dparams_d, const float* dlandmar
                                    float* dw1_d, float* db1_d, float* dw2_d, float* db2_d, void* workspace_d,
                                    size_t workspace_bytes, dad3d_stream stream);
 
+/* ---- UV textures: the demo's uv_texture output for every boxed head ------------------------------------------------------
+ *   Replace UVTextureCreator._compute_texture_map (inference/uv_texture.py:21-47) with psbody's
+ *   Mesh.estimate_vertex_normals (face normals cross(v1 - v0, v2 - v0) summed per vertex in ascending face index, divided by
+ *   their norm, a norm of 0 replaced by 1), in fp64 as psbody's float64 Mesh.v.
+ *   dad3d_uv_create  uploads the compacted texture table to `device`: entry e writes texel texel_h[e] (y * img_size + x, all
+ *     distinct, in [0, img_size^2)) from vertex_ids_h [T,3] (in [0, V)) with barycentrics bary_h [T,3]; faces_h [NF,3] are
+ *     the mesh's faces and csr_row_h [V+1] / csr_col_h [nnz] the rows of faces_by_vertex(as_sparse_matrix=True): each
+ *     vertex's distinct faces, ascending.  A face listing a vertex twice counts twice, as the CSR's summed entries do.
+ *   dad3d_uv_workspace_bytes  scratch of dad3d_uv_texture for R heads (0 for a null handle or R < 0).  After a call it
+ *     holds [R,V] fp64, the normalised vertex normals' z of every head that ran (valid, frame in range).
+ *   dad3d_uv_texture  vertices_d [R,V,3] fp32 (frame pixels with depth: projected_vertices of to_2d=False) of heads on
+ *     frames_d [F,H,W,3] uint8 (head r on frame frame_index_d[r]; null: frame 0) -> out_d [R,img_size,img_size,3] uint8, the
+ *     reference's texture of each head: texels facing the view (n_dot_view >= 0 or NaN) whose rounded (half to even) point
+ *     lies strictly inside (0, W) x (0, H) copy that frame pixel, every other texel is 0.  A head with valid_d[r] == 0 (null:
+ *     all valid) or a frame index outside [0, F) gets an all-zero texture.  2 kernels for R from 1 to 65 535; none for
+ *     R == 0.  No host synchronisation. */
+typedef struct dad3d_uv dad3d_uv;
+DAD3D_API int dad3d_uv_create(dad3d_uv** out, int32_t img_size, const int32_t* texel_h, const int32_t* vertex_ids_h,
+                              const double* bary_h, int32_t T, const int32_t* faces_h, int32_t NF, const int32_t* csr_row_h,
+                              const int32_t* csr_col_h, int32_t V, int32_t device);
+DAD3D_API void dad3d_uv_destroy(dad3d_uv* h);
+DAD3D_API size_t dad3d_uv_workspace_bytes(const dad3d_uv* h, int32_t R);
+DAD3D_API int dad3d_uv_texture(const dad3d_uv* h, const float* vertices_d, int32_t R, const uint8_t* valid_d,
+                               const uint8_t* frames_d, int32_t F, int32_t H, int32_t W, const int32_t* frame_index_d,
+                               uint8_t* out_d, void* workspace_d, size_t workspace_bytes, dad3d_stream stream);
+
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 DAD3D_API unsigned long long dad3d_launch_count(void);
 
